@@ -115,7 +115,7 @@ def lib():
     global _lib
     if _lib is None:
         if not os.path.exists(LIB_PATH):
-            raise ImportError("libagp.so is not built: run `python __graft_entry__.py` (nvcc, sm_100a). "
+            raise ImportError("libagp.so is not built: run `python __graft_entry__.py` (nvcc, sm_90a). "
                               "There is no CPU fallback.")
         try:  # make the torch-bundled libnccl visible first if torch is importable (same SONAME)
             import torch  # noqa: F401

@@ -45,7 +45,7 @@ struct agp_ctx {
   int profile = 1;
   int rank = 0, nranks = 1, grid_p = 1, grid_q = 1;
   ncclComm_t nccl = nullptr;
-  OzakiWs oz{};            // slice workspace of the tcgen05 fp64 path (cached across fits of the same shape)
+  OzakiWs oz{};            // slice workspace of the int8-slice fp64 path (cached across fits of the same shape)
   OzakiWs oz2{};           // second slice buffer of the pipelined distributed schedule (panel k+1 is sliced while rest(k) runs)
   int64_t oz_rows = 0, oz2_rows = 0;
   cudaStream_t stream_comm = nullptr;  // panel broadcasts of the pipelined distributed schedule
@@ -218,7 +218,7 @@ void trailing_update(agp_ctx* ctx, T* L, int64_t lda, int64_t row0, int64_t col0
   if (M <= 0 || N <= 0) return;
   if (ctx->profile) cudaEventRecord(prof_event(ctx), st);
   bool done = false;
-  if (oz) {  // tcgen05 int8-sliced path: the slices of panel rows [oz_row0, ...) are already in *oz
+  if (oz) {  // int8-sliced tensor-core path: the slices of panel rows [oz_row0, ...) are already in *oz
     if constexpr (std::is_same<T, double>::value) {
       ozaki_syrk(*oz, L + row0 + col0 * lda, lda, M, N, 1, 0, 0, col0 - oz_row0, row0 - oz_row0, st);
       done = true;
@@ -247,7 +247,7 @@ static void join_inverses(agp_ctx* ctx) {
 }
 
 // resolve the outer panel width (in 128-blocks) and the fp64 trailing-update engine for a problem size:
-// explicit config / env wins; "auto" = tcgen05 int8-sliced path with 512-wide panels from n_pad >= 8192
+// explicit config / env wins; "auto" = int8-sliced tensor-core path with 512-wide panels from n_pad >= 8192
 static int resolve_G(const agp_ctx* ctx, int64_t n_pad) {
   int nb = ctx->cfg.tile_nb;
   if (nb <= 0) nb = (n_pad >= 8192) ? 512 : TILE;
@@ -259,7 +259,7 @@ static int resolve_fp64_mode(const agp_ctx* ctx, int64_t n_pad) {
   if (ctx->cfg.fp64_mode >= 0) return ctx->cfg.fp64_mode;
   return n_pad >= 8192 ? 1 : 0;
 }
-// fp32: 0 = FFMA tile kernels, 1 = int8-sliced tcgen05 path (4 slices); auto = tcgen05 from n_pad >= 4096
+// fp32: 0 = FFMA tile kernels, 1 = int8-sliced tensor-core path (4 slices); auto = int8 slices from n_pad >= 4096
 static int resolve_fp32_mode(const agp_ctx* ctx, int64_t n_pad) {
   if (ctx->cfg.fp32_mode >= 0) return ctx->cfg.fp32_mode;
   return n_pad >= 4096 ? 1 : 0;
@@ -352,7 +352,7 @@ void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t ro
                       double* logdet_part, int* info) {
   cudaStream_t s = ctx->stream, s2 = ctx->stream2;
   const int nblk = (int)(n_pad / TILE);
-  const int fp64_mode = resolve_tensor_mode<T>(ctx, n_pad);  // 1: int8-sliced tcgen05 trailing update (fp64: 7 slices, fp32: 4)
+  const int fp64_mode = resolve_tensor_mode<T>(ctx, n_pad);  // 1: int8-sliced tensor-core trailing update (fp64: 7 slices, fp32: 4)
   int G = resolve_G(ctx, n_pad);
   if (!std::is_same<T, double>::value && fp64_mode == 1 && ctx->cfg.tile_nb <= 0 && n_pad >= 4096) G = 4;  // 512-wide panels
   const bool oz_ok = fp64_mode == 1 && nblk > 2 * G && ensure_oz(ctx, rows_total, G * TILE, slices_of<T>(ctx), s) &&
@@ -370,7 +370,7 @@ void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t ro
     if (cols_trail <= 0) continue;
     const int64_t K = (int64_t)(g_end - ko) * TILE, kc0 = (int64_t)ko * TILE;
     const OzakiWs* oz = nullptr;
-    // tcgen05 path: needs the full outer-panel width it was sized for and enough trailing work to pay for slicing
+    // int8-slice path: needs the full outer-panel width it was sized for and enough trailing work to pay for slicing
     if (oz_ok && K == ctx->oz.K && cols_trail >= 2 * TILE) oz = &ctx->oz;
     constexpr int is_f32 = std::is_same<T, double>::value ? 0 : 1;
     if (!la) {
@@ -379,14 +379,14 @@ void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t ro
       continue;
     }
     if (la2 && !oz) {
-      // EXPERIMENTAL look-ahead depth 2 (cfg.lookahead = 2 / AGP_LOOKAHEAD=2, DMMA path only -- the tcgen05 path would
+      // EXPERIMENTAL look-ahead depth 2 (cfg.lookahead = 2 / AGP_LOOKAHEAD=2, DMMA path only -- the int8-slice path would
       // need a second slice buffer; not yet run on a device).  The rest update is split: restA = the panel after next,
       // restB = everything beyond.  The next-panel update of step k+1 needs only restA(k), so the latency-bound chain
       // (potrf -> TRSM -> next-panel update) no longer waits for the bulk of the previous rest update; restB(k) has two
       // chain steps to finish instead of one (it is serialised behind restB(k-1) and restA(k) on the side stream).
       cudaEvent_t e_panel = dep_event(ctx, ev_idx++), e_restA = dep_event(ctx, ev_idx++), e_restB = dep_event(ctx, ev_idx++);
       if (restA_pending) cudaStreamWaitEvent(s, dep_event(ctx, last_restA), 0);
-      // a previous step may have used the depth-1 branch (tcgen05 panel followed by a short DMMA tail): its rest update
+      // a previous step may have used the depth-1 branch (int8-slice panel followed by a short DMMA tail): its rest update
       // on the side stream touches the same block column as the update below
       if (rest_pending && last_rest_full) cudaStreamWaitEvent(s, dep_event(ctx, last_rest), 0);
       cudaEventRecord(e_panel, s);
@@ -438,7 +438,7 @@ void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t ro
 // V <- L^-1 V on the tensor cores: two-level blocked substitution.  Inside an outer block of W = 512 rows the 128-step
 // loop runs on the tile GEMMs (W^2 ncols work); everything below the block receives ONE rank-W update
 //   B[below] -= L[below, block] * B[block]
-// on the int8-sliced tcgen05 kernel: the L panel (rows_below x W, row-contiguous) and B[block]' (ncols x W, k-major) are
+// on the int8-sliced tensor-core kernel: the L panel (rows_below x W, row-contiguous) and B[block]' (ncols x W, k-major) are
 // sliced into one workspace (A rows first, B rows behind them) and the product is a rectangular update of B[below].
 // This is `C.U' \ X` of /root/reference/src/util/common_covmat_ops.jl:54,90 (prediction, N^2 M flops at config C3) and the
 // A = U' \ K_zx solve of /root/reference/src/sparse_approximations.jl:296.
@@ -1900,7 +1900,7 @@ int fit_dist_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
   // pipelined schedule: 1 = the owner of the next panel runs its rest update AFTER that panel's factorisation; 0 = at once
   // (bounded CTAs + stream priorities let the factorisation through)
   const bool dist_defer = env_int64("AGP_DIST_DEFER", 1) != 0;
-  int nsm_dev = 148;
+  int nsm_dev = 0;
   cudaDeviceGetAttribute(&nsm_dev, cudaDevAttrMultiProcessorCount, ctx->device);
   struct DeferredRest { bool on; int kk; T* Pk; int lo, hi; bool use_oz; cudaEvent_t e_rest; };
   DeferredRest def{false, 0, nullptr, 0, 0, false, nullptr};
@@ -2158,7 +2158,7 @@ int env_int(const char* name, int dflt) {
 
 extern "C" {
 
-const char* agp_version(void) { return "agp-blackwell 0.1 (sm_100a)"; }
+const char* agp_version(void) { return "agp-blackwell 0.1 (sm_90a)"; }
 
 int32_t agp_init(agp_ctx** out, int32_t device, const agp_config* cfg) {
   if (!out) return AGP_ERR_INVALID;
@@ -2173,7 +2173,7 @@ int32_t agp_init(agp_ctx** out, int32_t device, const agp_config* cfg) {
   if (ctx->cfg.tile_nb % TILE) ctx->cfg.tile_nb = 0;
   ctx->cfg.fp64_mode = env_int("AGP_FP64_MODE", cfg ? ctx->cfg.fp64_mode : -1);            // -1 = auto
   ctx->cfg.fp32_mode = env_int("AGP_FP32_MODE", cfg ? ctx->cfg.fp32_mode : -1);            // -1 = auto
-  ctx->cfg.lookahead = env_int("AGP_LOOKAHEAD", cfg ? ctx->cfg.lookahead : 2);  // 2: depth-2 look-ahead on the DMMA path (validated in round 2: C2 3.49 -> 3.27 ms)
+  ctx->cfg.lookahead = env_int("AGP_LOOKAHEAD", cfg ? ctx->cfg.lookahead : 2);  // 2: depth-2 look-ahead on the DMMA path
   ctx->cfg.use_graph = env_int("AGP_GRAPH", ctx->cfg.use_graph);
   ctx->profile = env_int("AGP_PROFILE", cfg ? cfg->profile_kernels : 0);
   ctx->oz_S = env_int("AGP_OZAKI_S", (cfg && cfg->ozaki_slices) ? cfg->ozaki_slices : 7);
@@ -2362,7 +2362,6 @@ int32_t agp_debug_ozaki_syrk(agp_ctx* ctx, void* C_dev, int64_t ldc, const void*
   OzakiWs ws;
   int rc = ozaki_ws_create(&ws, M, K, S, ctx->stream);
   if (rc) { ctx->err = "ozaki_ws_create failed (code " + std::to_string(rc) + ")"; return rc == 1 ? AGP_ERR_INVALID : AGP_ERR_CUDA; }
-  if (!(lower_only && N % 128 == 0 && N >= 128)) ws.bulk = 0;  // the non-persistent kernel reads the row-major slice layout
   ozaki_prepare(ws, (const double*)P_dev, lda, M, ctx->stream);
   ozaki_syrk(ws, (double*)C_dev, ldc, M, N, lower_only, 0, 0, 0, 0, ctx->stream);
   ozaki_ws_destroy(&ws, ctx->stream);
@@ -2372,7 +2371,7 @@ int32_t agp_debug_ozaki_syrk(agp_ctx* ctx, void* C_dev, int64_t ldc, const void*
   return AGP_OK;
 }
 
-// general product on the tcgen05 path: C (M x N, fp32 or fp64) += sign * A B', A = M x K, B = N x K (B_dev == NULL: B = A,
+// general product on the int8-slice path: C (M x N, fp32 or fp64) += sign * A B', A = M x K, B = N x K (B_dev == NULL: B = A,
 // lower tiles only).  Each operand is fp32 or fp64, row-contiguous (element (r, k) at [r + k*ld]) or k-major ([k + r*ld]).
 // Both operands are sliced into one workspace (A rows first, B rows from the next multiple of 128).
 int32_t agp_debug_ozaki_gemm(agp_ctx* ctx, void* C_dev, int32_t c_is_float, int64_t ldc, const void* A_dev, int32_t a_is_float,

@@ -7,7 +7,7 @@
 // fp64: 128x128x16 CTA tile, 3-stage cp.async pipeline, 8 warps x (64x32) warp tiles of
 //       mma.sync.m8n8k4.f64 (DMMA) -- padded smem strides make every fragment load conflict-free.
 // fp32: 128x128x16 CTA tile, register-prefetch double buffering, 8x8 FFMA micro-tiles.
-// The tcgen05 kernels (umma_*.cu) replace these on the trailing update when enabled.
+// The int8-slice wgmma kernel (umma_ozaki.cu) replaces these on the trailing update when enabled.
 #include "kernels.h"
 #include "agp.h"
 

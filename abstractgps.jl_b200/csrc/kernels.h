@@ -1,4 +1,4 @@
-// kernels.h -- launch-level interface between the engine (engine.cu) and the sm_100a kernels.
+// kernels.h -- launch-level interface between the engine (engine.cu) and the sm_90a kernels.
 // All matrices are column-major.  TILE = 128 is the factorisation tile edge: every matrix the
 // Cholesky touches is padded to a multiple of TILE (identity padding), so kernels on that path
 // see no ragged edges; the generic GEMM still bounds-checks for the prediction path.

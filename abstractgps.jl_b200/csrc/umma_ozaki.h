@@ -1,4 +1,4 @@
-// umma_ozaki.h -- host interface of the tcgen05 int8-sliced (Ozaki) fp64 trailing update
+// umma_ozaki.h -- host interface of the int8-sliced (Ozaki) trailing update on the Hopper tensor cores (wgmma)
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -11,15 +11,13 @@ struct OzakiWs {
   int64_t m_alloc;  // rows per slice (multiple of 128)
   int K;            // panel width (bytes per slice row), multiple of 64
   int S;            // number of 7-bit slices (5..8)
-  CUtensorMap tmap; // 2-D uint8 tensor (K, S*m_alloc), box 64 B x 64 rows, 64-byte swizzle (v1 kernel)
-  int bulk;   // 2: slices in the blocked UMMA layout [row block][k block][slice] fetched with 1-D bulk copies (persistent kernel);
-              // 0: row-major slices behind the tensor map (non-persistent kernel, generic shapes)
-  int64_t* tab_start;  // device tables of the block-cyclic tile enumeration (v2), two slots of tab_cap+1 entries:
+  int bulk;   // 2: slices in the blocked no-swizzle K-major layout [row block][k block][slice] fetched with 1-D bulk copies
+  int64_t* tab_start;  // device tables of the block-cyclic tile enumeration  of tab_cap+1 entries:
   int32_t* tab_bimin;  // consecutive calls (main / side stream) alternate slots
   int tab_cap;
   mutable int tab_slot;
-  mutable int chunk_tiles;  // v3 kernel: > 0 -> bounded CTAs of this many consecutive tiles (see the kernel), 0 -> persistent
-  mutable int max_ctas;  // persistent (v2) kernel: cap on the grid, 0 = one CTA per SM.  The distributed schedule leaves
+  mutable int chunk_tiles;  // > 0 -> bounded CTAs of this many consecutive tiles (see the kernel), 0 -> persistent
+  mutable int max_ctas;  // persistent kernel: cap on the grid, 0 = one CTA per SM.  The distributed schedule leaves
                          // a few SMs to the NCCL broadcast that overlaps the update.
 };
 
@@ -33,12 +31,12 @@ void ozaki_prepare(const OzakiWs& ws, const double* P, int64_t lda, int64_t m, c
 void ozaki_syrk(const OzakiWs& ws, double* C, int64_t ldc, int64_t M, int64_t N, int lower_only, int64_t b_tile_stride,
                 int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s);
 
-// generalised entry points (v3 kernel, interleaved slice layout only):
+// generalised entry points:
 //  * operands may be fp32 or fp64, row-contiguous (element (row, k) at P[row + k*lda]) or k-major (P[k + row*lda]); the
 //    rows land at [dst_row0, dst_row0 + m) of the slice buffer (dst_row0 a multiple of 128), so the two operands of a general
 //    product C += sign * A B' are sliced into ONE workspace and addressed with a_off / b_off;
 //  * C may be fp32 or fp64; full = 1: every row tile of every 64-column strip (rectangular product), 0: lower tiles only.
-// returns 0 on success, 1 if the workspace / shape is not supported by the v3 path.
+// returns 0 on success, 1 if the workspace / shape is not supported.
 void ozaki_prepare_ex(const OzakiWs& ws, const void* P, int p_is_float, int kmajor, int64_t lda, int64_t m, int64_t dst_row0,
                       cudaStream_t s);
 int ozaki_update_ex(const OzakiWs& ws, void* C, int c_is_float, int64_t ldc, int64_t M, int64_t N, int full, double sign,

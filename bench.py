@@ -4,9 +4,10 @@ ms to logpdf(fx,y) + posterior(fx,y) at N x D fp64, with the achieved fraction o
 trailing update and of the N^3/3 Cholesky rate, next to the reference's CPU LAPACK path timed on the same box.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--workload C4|C2|C4h|C3|C5] [--impl ours|reference] [--n N]
+                  [--dump-outputs DIR]
 
 The SAME workload (C4: N = 65 536, D = 64, SqExponential, fp64 -- the configuration BASELINE.json's metric and target are
-quoted on; it fits one B200) runs at every --gpus value, so the per-N values form a strong-scaling curve.  At N = 1 the
+quoted on; 34 GB, it fits one 80 GB H100) runs at every --gpus value, so the per-N values form a strong-scaling curve.  At N = 1 the
 line also carries C2 (N = 4096, D = 8) as the secondary key "c2".
 
 One "step" = one pass of the hot path through the C ABI of libagp.so:
@@ -16,6 +17,9 @@ One "step" = one pass of the hot path through the C ABI of libagp.so:
 HOST buffers, H2D/D2H inside the timed region.  Device times come from CUDA events recorded by the library on its
 launching stream, max over ranks.  The oracle (oracle/agp_ref.py) is used here only as the CPU baseline and as the
 out-of-timed-region parity checker.
+--dump-outputs DIR writes what the last timed step returned to its caller (logpdf / elbo, the posterior weights alpha,
+the predictive mean and variance) as DIR/<name>.npy; the inputs are generated from fixed seeds, so two builds can be
+compared output for output.
 """
 from __future__ import annotations
 
@@ -61,7 +65,7 @@ def wl_string(wl, N, extra=""):
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons DURING the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons DURING the timed region."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
          "clocks_event_reasons.sw_power_cap")
@@ -124,7 +128,7 @@ def trailing_flops(N, nb=128):
 # ------------------------------------------------------------------------------------------------------------
 def cpu_step(wl, cfg):
     """One step of the reference's CPU algorithm for the workload (oracle port).  fit: logpdf THEN posterior -- TWO Gram
-    builds and TWO LAPACK potrf's, as /root/reference/src/finite_gp_projection.jl:307-308 + src/exact_gpr_posterior.jl:30-31
+    builds and TWO LAPACK potrf's, as the reference's src/finite_gp_projection.jl:307-308 + src/exact_gpr_posterior.jl:30-31
     do; the Distances.jl (gemm) pairwise formulation the reference executes."""
     from oracle import agp_ref as ref
     kind = WORKLOADS[wl]["kind"]
@@ -228,13 +232,6 @@ def run_reference(args, wl, n_full):
 # ------------------------------------------------------------------------------------------------------------
 # GPU side
 # ------------------------------------------------------------------------------------------------------------
-def load_peaks():
-    try:
-        return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-        return {}
-
-
 def measure_dgemm_peak(torch, dev):
     """native fp64 reference rate: cuBLAS DGEMM 8192^3 on this box, best of 5 (CUDA events)."""
     n = 8192
@@ -254,47 +251,8 @@ def measure_dgemm_peak(torch, dev):
     return 2.0 * n ** 3 / (best * 1e-3) / 1e12
 
 
-def measure_int8_mma_peak(eng, torch, dev, S=7):
-    """MEASURED int8 tcgen05 rate of this kernel's own instruction mix: the persistent trailing-update kernel run with
-    its operand traffic and epilogue switched off (probe mode 5: every tile still issues all of its tcgen05.mma.kind::i8
-    instructions on operands already in shared memory).  TOP/s = executed int8 ops / time, slicing time subtracted."""
-    import ctypes as C
-    M, K = 16384, 512
-    P = torch.randn(K, M, dtype=torch.float64, device=dev)
-    Cm = torch.zeros(M, M, dtype=torch.float64, device=dev)
-    old = os.environ.get("AGP_OZAKI_EPI")
-
-    def run(ncols):
-        best = 1e9
-        for _ in range(3):
-            torch.cuda.synchronize()
-            t0 = time.perf_counter()
-            eng.check(eng.L.agp_debug_ozaki_syrk(eng.h, C.c_void_p(Cm.data_ptr()), M, C.c_void_p(P.data_ptr()), M, M, ncols, K, S, 1))
-            best = min(best, time.perf_counter() - t0)
-        return best
-    try:
-        os.environ["AGP_OZAKI_EPI"] = "5"
-        fixed = run(128)
-        full = run(M)
-    finally:
-        if old is None:
-            os.environ.pop("AGP_OZAKI_EPI", None)
-        else:
-            os.environ["AGP_OZAKI_EPI"] = old
-    nbi, nbj = M // 128, M // 64
-    tiles = sum(min(nbj, 2 * bi + 2) for bi in range(nbi)) - 2  # minus the strip of the `fixed` run (approx.)
-    ops = 2.0 * tiles * 128 * 64 * K * (S * (S + 1) // 2)
-    del P, Cm
-    return ops / max(full - fixed, 1e-9) / 1e12
-
-
-def ncu_traffic(tag):
-    """dram__bytes_read.sum + dram__bytes_write.sum of one launch of the dominant kernel from the committed ncu capture
-    under profiles/ (see profiles/README.md), with that launch's algorithmic bytes -- None when no capture is committed."""
-    try:
-        return json.load(open(os.path.join(ROOT, "profiles", "traffic.json")))[tag]
-    except Exception:
-        return None
+INT8_PEAK_TOPS = 1979.0  # NVIDIA H100 SXM data sheet, dense int8 tensor rate at up to 700 W (a share-of-peak denominator)
+FP32_PEAK_TFLOPS = 67.0  # same data sheet, fp32 (FFMA)
 
 
 class FitProblem:
@@ -416,7 +374,7 @@ def timed(prob, torch, flush, device_resident, steps, warmup, dist=None):
 
 def parity_check(wl, prob_cls_args, eng, torch, dev, dist=None):
     """out-of-timed-region parity of the BENCHED path against the oracle: the workload itself when N <= 8192, else its
-    first 8192 points through the same engine configuration (n_pad >= 8192 keeps the tcgen05 / distributed path)."""
+    first 8192 points through the same engine configuration (n_pad >= 8192 keeps the int8-slice tensor-core / distributed path)."""
     from oracle import agp_ref as ref
     W = WORKLOADS[wl]
     n_full = prob_cls_args["n"]
@@ -453,7 +411,6 @@ def fit_roofline(wl, N, eng, torch, dev, prob, flush, args, world=1, dist=None, 
     """roofline of the dominant kernel = the outer trailing update.  Its launches are timed with CUDA events around every
     launch inside the library (profile_kernels = 1); on one GPU the look-ahead schedule overlaps two of them on two
     streams, so that pass runs with look-ahead OFF (serial launches), same inputs, same kernels."""
-    peaks = load_peaks()
     cfg0 = eng.get_config()
     W = WORKLOADS[wl]
     if dist is None:
@@ -478,16 +435,10 @@ def fit_roofline(wl, N, eng, torch, dev, prob, flush, args, world=1, dist=None, 
         pairs = S_sl * (S_sl + 1) // 2
         fp64_eq = tf / world / (trailing_ms * 1e-3) / 1e12 if trailing_ms > 0 else None  # per GPU
         achieved = fp64_eq * pairs if fp64_eq else None  # executed int8 TOP/s per GPU: every fp64 MAC = S(S+1)/2 int8 MACs
-        mma_peak = measure_int8_mma_peak(eng, torch, dev, S_sl)
-        nominal = 4500.0
-        out.update({"bound": "tensor", "kernel": "umma_ozaki_syrk_v2_kernel<%d> (tcgen05.mma.kind::i8, TMA, TMEM; persistent)" % S_sl,
-                    "achieved": achieved, "peak": mma_peak, "unit": "TOP/s (int8 tensor, dense, per GPU)",
-                    "frac": (achieved / mma_peak) if achieved else None,
-                    "peak_source": "MEASURED in this run: the same kernel's tcgen05.mma.kind::i8 instruction stream with operand traffic and "
-                                   "epilogue off (operands resident in shared memory), 16384 x 16384 x 512 -- the tensor-pipe ceiling of this "
-                                   "instruction mix on this box",
-                    "frac_of_2x_bf16_measured": (achieved / (2.0 * peaks["bf16_tflops"])) if (achieved and "bf16_tflops" in peaks) else None,
-                    "frac_of_nominal_4500": (achieved / nominal) if achieved else None,
+        out.update({"bound": "tensor", "kernel": "ozaki_syrk_wgmma_kernel<%d> (wgmma s8 x s8 -> s32, bulk async copies)" % S_sl,
+                    "achieved": achieved, "peak": INT8_PEAK_TOPS, "unit": "TOP/s (int8 tensor, dense, per GPU)",
+                    "frac": (achieved / INT8_PEAK_TOPS) if achieved else None,
+                    "peak_source": "H100 SXM data sheet (dense int8, 700 W)",
                     "fp64_equivalent_tflops_per_gpu": fp64_eq, "slices": S_sl, "int8_macs_per_fp64_mac": pairs})
     elif W["dtype"] == "f64":
         dgemm = measure_dgemm_peak(torch, dev)
@@ -498,25 +449,19 @@ def fit_roofline(wl, N, eng, torch, dev, prob, flush, args, world=1, dist=None, 
     else:
         fp32 = tf / world / (trailing_ms * 1e-3) / 1e12 if trailing_ms > 0 else None
         f32_mode = cfg0.fp32_mode if cfg0.fp32_mode >= 0 else (1 if n_pad >= 4096 else 0)
-        if f32_mode == 1:  # the same int8-sliced tcgen05 kernel with 4 slices: 10 int8 MACs per fp32 MAC
+        if f32_mode == 1:  # the same int8-sliced wgmma kernel with 4 slices: 10 int8 MACs per fp32 MAC
             S32 = int(os.environ.get("AGP_OZAKI_S32", "4"))
             pairs = S32 * (S32 + 1) // 2
             achieved = fp32 * pairs if fp32 else None
-            mma_peak = measure_int8_mma_peak(eng, torch, dev, 7)
-            out.update({"bound": "tensor", "kernel": "umma_ozaki_syrk_v3_kernel<%d, ., ., ., float> (tcgen05.mma.kind::i8, fp32 operands in %d slices)" % (S32, S32),
-                        "achieved": achieved, "peak": mma_peak, "unit": "TOP/s (int8 tensor, dense, per GPU)",
-                        "frac": (achieved / mma_peak) if achieved else None,
-                        "peak_source": "MEASURED in this run: the fp64 (7-slice) instance of the same kernel with operand traffic and epilogue off",
-                        "frac_of_nominal_4500": (achieved / 4500.0) if achieved else None,
+            out.update({"bound": "tensor", "kernel": "ozaki_syrk_wgmma_kernel<%d, float> (wgmma s8 x s8 -> s32, fp32 operands in %d slices)" % (S32, S32),
+                        "achieved": achieved, "peak": INT8_PEAK_TOPS, "unit": "TOP/s (int8 tensor, dense, per GPU)",
+                        "frac": (achieved / INT8_PEAK_TOPS) if achieved else None,
+                        "peak_source": "H100 SXM data sheet (dense int8, 700 W)",
                         "fp32_equivalent_tflops_per_gpu": fp32, "slices": S32, "int8_macs_per_fp32_mac": pairs})
         else:
-            ffma_peak = 148 * 128 * 2 * 1.965e9 / 1e12
-            out.update({"bound": "fp32 FMA", "kernel": "gemm_simt_kernel (FFMA tiles)", "achieved": fp32, "peak": ffma_peak,
-                        "unit": "TFLOP/s (fp32)", "frac": (fp32 / ffma_peak) if fp32 else None,
-                        "peak_source": "nominal 148 SMs x 128 FFMA/clk x 2 x 1.965 GHz"})
-    tr = ncu_traffic(wl if wl in ("C4", "C4h", "C2", "C3", "C5") else "C4")
-    out["traffic"] = tr.get("dram_bytes_per_launch") if tr else None
-    out["traffic_detail"] = tr
+            out.update({"bound": "fp32 FMA", "kernel": "gemm_simt_kernel (FFMA tiles)", "achieved": fp32, "peak": FP32_PEAK_TFLOPS,
+                        "unit": "TFLOP/s (fp32)", "frac": (fp32 / FP32_PEAK_TFLOPS) if fp32 else None,
+                        "peak_source": "H100 SXM data sheet (fp32, 700 W)"})
     if t_dev:
         chol_tf = (N ** 3 / 3.0) / (t_dev["cholesky"] * 1e-3) / 1e12
         out["cholesky_third_n3_tflops"] = chol_tf
@@ -550,12 +495,14 @@ def run_ours(args, wl, n_full):
         eng = ag.engine()
     prob = FitProblem(wl, n_full, eng, torch, dev)
     N, D = prob.N, prob.D
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)  # > 50 MB L2
 
     sampler = ClockSampler(local)
     if rank == 0:
         sampler.start()
     t_dev, wall_dev, launches = timed(prob, torch, flush, True, args.steps, args.warmup, dist)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(prob, args.dump_outputs)
     if args.quick:  # development runs (schedule sweeps): device-resident timing only, no e2e / parity / roofline / CPU arm
         if rank == 0:
             sampler.stop()
@@ -592,20 +539,19 @@ def run_ours(args, wl, n_full):
         if tensor:
             S_ = int(os.environ.get("AGP_OZAKI_S32", "4")) if W["dtype"] == "f32" else cfg0.ozaki_slices
             pairs = S_ * (S_ + 1) // 2
-            mma_peak = measure_int8_mma_peak(eng, torch, dev, 7)
             ach = 2.0 * M * M * N / world * pairs / (stream_ms * 1e-3) / 1e12  # executed int8 TOP/s per GPU (TRSM + SYRK = M^2 N MACs)
-            roofline = {"bound": "tensor", "kernel": "umma_ozaki_syrk_v3_kernel (TRSM rank-512 updates + long-K SYRK accumulate, %d slices)" % S_,
-                        "achieved": ach, "peak": mma_peak, "unit": "TOP/s (int8 tensor, dense, per GPU)", "frac": ach / mma_peak,
-                        "peak_source": "MEASURED in this run: the 7-slice instance of the same kernel with operand traffic and epilogue off",
-                        "frac_of_nominal_4500": ach / 4500.0, "alg_flops_per_step": alg, "kernel_ms_per_step": stream_ms,
+            roofline = {"bound": "tensor", "kernel": "ozaki_syrk_wgmma_kernel (TRSM rank-512 updates + long-K SYRK accumulate, %d slices)" % S_,
+                        "achieved": ach, "peak": INT8_PEAK_TOPS, "unit": "TOP/s (int8 tensor, dense, per GPU)", "frac": ach / INT8_PEAK_TOPS,
+                        "peak_source": "H100 SXM data sheet (dense int8, 700 W)",
+                        "alg_flops_per_step": alg, "kernel_ms_per_step": stream_ms,
                         "fp_equivalent_tflops_whole_job": alg / (t_dev["total"] * 1e-3) / 1e12, "traffic": None,
                         "note": "kernel_ms = the whole streamed phase (cross-Gram, scaling, TRSM, SYRK, reductions), so frac is a lower bound for the kernel"}
         else:
-            ffma_peak = 148 * 128 * 2 * 1.965e9 / 1e12 * world
+            ffma_peak = FP32_PEAK_TFLOPS * world
             ach = alg / (t_dev["total"] * 1e-3) / 1e12
             roofline = {"bound": "fp32 FMA", "kernel": "VFE stream on the tile GEMMs", "achieved": ach, "peak": ffma_peak,
                         "unit": "TFLOP/s (whole job)", "frac": ach / ffma_peak, "alg_flops_per_step": alg,
-                        "peak_source": "nominal N_gpus x 148 SMs x 128 FMA/clk x 2 x 1.965 GHz", "traffic": None}
+                        "peak_source": "H100 SXM data sheet (fp32, 700 W) x N_gpus", "traffic": None}
     if rank != 0:
         return
     cpu = cpu_baseline(wl, n_full)
@@ -626,6 +572,20 @@ def run_ours(args, wl, n_full):
     if wl == "C4" and world == 1 and not args.no_c2:
         line["c2"] = secondary_c2(eng, torch, dev, flush, args)
     print(json.dumps(line))
+
+
+def dump_outputs(prob, out_dir):
+    """what the last timed step returned to its caller, as DIR/<name>.npy (float32 / float64, the workload's dtype)"""
+    os.makedirs(out_dir, exist_ok=True)
+    prob.torch.cuda.synchronize()
+    if prob.kind == "vfe":
+        outs = {"elbo": prob.lp[0:1], "dtc": prob.lp[1:2]}
+    else:
+        outs = {"logpdf": prob.lp[0:1], "alpha": prob.alpha_d.cpu().numpy()}
+        if prob.kind == "fit_predict":
+            outs.update(mean=prob.mu_d.cpu().numpy(), var=prob.var_d.cpu().numpy())
+    for name, a in outs.items():
+        np.save(os.path.join(out_dir, name + ".npy"), np.array(a, dtype=prob.np_dt))
 
 
 def secondary_c2(eng, torch, dev, flush, args):
@@ -654,6 +614,8 @@ def main():
     ap.add_argument("--n", type=int, default=None, help="override N of the workload (development / shard-sized runs)")
     ap.add_argument("--no-c2", action="store_true", help="skip the secondary C2 measurement on the N=1 C4 line")
     ap.add_argument("--quick", action="store_true", help="development: device-resident timing only (not a bench line)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy")
     args = ap.parse_args()
     if args.impl == "ours":
         args.warmup = max(args.warmup, 3)

@@ -1,5 +1,5 @@
 /* Minimal C client of the drop-in boundary (include/agp.h): logpdf + posterior weights from ONE call, then a
- * predictive mean/variance at the training points.  Build (the library itself needs a B200 to run):
+ * predictive mean/variance at the training points.  Build (the library itself needs an H100 to run):
  *   gcc -std=c99 -Iinclude examples/c_abi_demo.c -o c_abi_demo -Labstractgps.jl_b200 -l:libagp.so -lm
  * This is what the reference-side binding (julia/AGPBlackwell.jl, `ccall`) does, in C. */
 #include <math.h>

@@ -1,4 +1,4 @@
-/* agp.h -- C ABI of libagp.so, the Blackwell-native (sm_100a) exact-GP engine that sits
+/* agp.h -- C ABI of libagp.so, the Hopper-native (sm_90a) exact-GP engine that sits
  * behind AbstractGPs.jl's dense hot path.
  *
  * The reference (pure Julia, /root/reference) has no FFI; the two seams a drop-in uses are
@@ -74,14 +74,14 @@ typedef struct {
 
 typedef struct {
   int32_t tile_nb;       /* OUTER panel width (multiple of 128); 0 -> auto (512 from n_pad >= 8192, else 128) */
-  int32_t fp64_mode;     /* -1 auto (tcgen05 from n_pad >= 8192), 0 = DMMA mma.sync trailing update,
-                            1 = int8-sliced (Ozaki) trailing update on tcgen05.mma.kind::i8 */
-  int32_t fp32_mode;     /* -1 auto (tcgen05 from n_pad >= 4096), 0 = FFMA tile kernels, 1 = int8-sliced trailing update /
-                            triangular solves on tcgen05.mma.kind::i8 (4 seven-bit slices cover the fp32 significand) */
+  int32_t fp64_mode;     /* -1 auto (int8 slices from n_pad >= 8192), 0 = DMMA mma.sync trailing update,
+                            1 = int8-sliced (Ozaki) trailing update on wgmma s8 x s8 */
+  int32_t fp32_mode;     /* -1 auto (int8 slices from n_pad >= 4096), 0 = FFMA tile kernels, 1 = int8-sliced trailing update /
+                            triangular solves on wgmma s8 x s8 (4 seven-bit slices cover the fp32 significand) */
   int32_t lookahead;     /* 0 off, 1: overlap the next panel with the bulk of the trailing update, 2 (default): additionally
                             split the bulk so that the chain waits only for the panel-after-next block (DMMA path) */
   int32_t use_graph;     /* reserved */
-  int32_t ozaki_slices;  /* 5..8 seven-bit slices of the tcgen05 fp64 path; 0 -> 7 (~2^-49 of the row scale) */
+  int32_t ozaki_slices;  /* 5..8 seven-bit slices of the int8 fp64 path; 0 -> 7 (~2^-49 of the row scale) */
   int32_t profile_kernels; /* 1: CUDA events around every trailing-update launch (agp_last_timings[7]); default 0 */
   int32_t reserved[9];
 } agp_config; /* NULL -> defaults; env AGP_NB, AGP_FP64_MODE, AGP_FP32_MODE, AGP_LOOKAHEAD, AGP_OZAKI_S, AGP_OZAKI_S32 override at agp_init */
@@ -208,12 +208,12 @@ int32_t agp_vfe_post_free(agp_vfe_post* p);
 /* Device-pointer entry points (AGP_MEM_DEVICE and the agp_debug_* hooks): the library runs on its OWN non-blocking streams
  * and returns after synchronising them, so results are complete on return -- but the CALLER must make sure the device
  * buffers it passes in are complete (synchronise the stream that produced them) before the call. */
-/* ---- test hook for the tcgen05 int8-sliced fp64 trailing update (csrc/umma_ozaki.cu): DEVICE pointers;
+/* ---- test hook for the int8-sliced fp64 trailing update (csrc/umma_ozaki.cu): DEVICE pointers;
  * C (M x N, ldc, fp64) -= P P' (lower tiles when lower_only), P = M x K fp64 (lda), S in 5..8 slices. */
 int32_t agp_debug_ozaki_syrk(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* P_dev, int64_t lda, int64_t M,
                              int64_t N, int32_t K, int32_t S, int32_t lower_only);
 
-/* general product on the same tcgen05 path: C (M x N, N % 128 == 0) += sign * A B' with fp32 or fp64 operands and output,
+/* general product on the same int8-slice path: C (M x N, N % 128 == 0) += sign * A B' with fp32 or fp64 operands and output,
  * row-contiguous (element (r,k) at [r + k*ld]) or k-major ([k + r*ld]) operands; B_dev == NULL: B = A, lower tiles only.
  * S = number of 7-bit slices (3..5 for fp32 output, 4..8 for fp64). */
 int32_t agp_debug_ozaki_gemm(agp_ctx* ctx, void* C_dev, int32_t c_is_float, int64_t ldc, const void* A_dev, int32_t a_is_float,

@@ -1,5 +1,5 @@
 # AGPBlackwell.jl -- the thin Julia shim a maintainer adds on the reference side so that AbstractGPs.jl's
-# dense hot path runs on libagp.so (hand-written sm_100a CUDA behind the C ABI of include/agp.h).
+# dense hot path runs on libagp.so (hand-written sm_90a CUDA behind the C ABI of include/agp.h).
 #
 # Julia is NOT available in the build image, so this file is shipped as source and has never been
 # executed (INTEGRATION.md lists what a maintainer should check first); every `ccall` below is mirrored 1:1 by the ctypes binding

@@ -65,7 +65,7 @@ def main():
             print("[rank %d] n=%d %s fam=%d: logpdf %s ref %s  ok=%s  posterior(mean_and_var, logdet, U) ok=%s  max|dmu|=%.3g max|dvar|=%.3g"
                   % (rank, n, np.dtype(dtype).name, fam, lp, lp_ref, good, good_p, np.abs(mu - mu_r).max(), np.abs(var - var_r).max()), flush=True)
         ok &= bool(good) and bool(good_p)
-    # a case large enough for the tcgen05 trailing update with the block-cyclic strip table (n_pad >= 8192, W = 512)
+    # a case large enough for the int8-slice trailing update with the block-cyclic strip table (n_pad >= 8192, W = 512)
     if os.environ.get("DIST_CHECK_LARGE", "1") == "1" and not only_stress:
         n, d = 8704, 8
         cfg = ref.make_config("C4", n=n)
@@ -93,7 +93,7 @@ def main():
         good &= np.allclose(mu, mu_r, rtol=1e-6, atol=1e-7) and np.allclose(var, var_r, rtol=1e-6, atol=1e-8)
         eng.L.agp_post_free(post)
         if rank == 0 or not good:
-            print("[rank %d] large n=%d (tcgen05 + strip table): logpdf %r ref %r ok=%s" % (rank, n, lp[0], lp_ref, bool(good)), flush=True)
+            print("[rank %d] large n=%d (int8 slices + strip table): logpdf %r ref %r ok=%s" % (rank, n, lp[0], lp_ref, bool(good)), flush=True)
         ok &= bool(good)
     # repeated fits at sizes where every rank owns few outer blocks (n_pad = a small multiple of 512 x ranks): steps are short,
     # so any missing dependency between the main-stream chain and the side-stream rest updates shows up as a wrong logpdf

@@ -1,7 +1,7 @@
 """Helper for tests/test_gpu_variants_grad_vfecov.py (run as a subprocess so that a device trap in an unvalidated kernel
-cannot poison the pytest process): runs the persistent tcgen05 SYRK with the default kernel and with the given
+cannot poison the pytest process): runs the int8-slice SYRK with the default (persistent) launch and with the given
 environment switches on the same inputs and prints the largest difference.
-Usage: python tests/exp_variant_check.py N K S AGP_OZAKI_CLUSTER=2 [AGP_OZAKI_EPIWARPS=8 ...]"""
+Usage: python tests/exp_variant_check.py N K S AGP_OZAKI_CHUNK_TEST=4 [AGP_OZAKI_EPI=0 ...]"""
 import ctypes as C
 import os
 import sys

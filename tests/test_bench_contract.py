@@ -42,14 +42,3 @@ def test_reference_arm_other_workloads_are_bounded():
     assert cfg["X"].shape[0] == 20000 and scale > 100 and "extrapolated" in sample
     cfg, scale, sample = bench.cpu_sample("C3", 16384)
     assert cfg["X"].shape[0] == 8192 and abs(scale - 8.0) < 1e-9 and cfg["Xs"].shape[0] == 5000
-
-
-def test_roofline_traffic_record_is_committed():
-    """bench.py fills roofline.traffic from the committed ncu capture of the benched workload (profiles/traffic.json)"""
-    sys.path.insert(0, ROOT)
-    import bench
-    for wl in ("C4", "C4h"):
-        t = bench.ncu_traffic(wl)
-        assert t and t["dram_bytes_per_launch"] > 0 and t["algorithmic_bytes_per_launch"] > 0
-        assert 1.0 <= t["ratio"] < 1.5, t["ratio"]          # traffic close to the algorithmic bytes: no wasted re-reads
-        assert os.path.exists(os.path.join(ROOT, t["capture"]))

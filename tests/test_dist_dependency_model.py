@@ -1,7 +1,7 @@
 """The pipelined multi-GPU schedule (fit_dist_impl, dist_sched == 2) replayed op by op on the CPU: every pair of operations
 of one rank that touch the same block column / panel buffer / slice buffer (at least one writing) must be ordered by stream
 order or an event edge.  tools/dist_dependency_model.py mirrors the enqueue order of csrc/engine.cu; with the
-`split_first` rule switched off it reproduces the race that surfaced on 8 ranks in round 2 (profiles/r02_call10_8gpu.log)."""
+`split_first` rule switched off it reproduces the race that once surfaced on 8 ranks."""
 import os
 import sys
 
@@ -12,7 +12,7 @@ sys.path.insert(0, os.path.join(ROOT, "tools"))
 import dist_dependency_model as m  # noqa: E402
 
 
-@pytest.mark.parametrize("use_oz", [True, False])  # tcgen05 path (updates read the slices) / DMMA-FFMA path (they read the panel)
+@pytest.mark.parametrize("use_oz", [True, False])  # int8-slice path (updates read the slices) / DMMA-FFMA path (they read the panel)
 @pytest.mark.parametrize("defer", [True, False])
 @pytest.mark.parametrize("R,nto", [(2, 4), (2, 9), (3, 10), (4, 11), (8, 16), (8, 17), (8, 5), (8, 33)])
 def test_shipped_schedule_has_no_unordered_conflicts(R, nto, defer, use_oz):

@@ -1,8 +1,6 @@
 """The event-graph of the distributed Cholesky (tools/dist_schedule_model.py mirrors the op order of fit_dist_impl):
-neither the default order nor the experimental AGP_DIST_SCHED=1 order may deadlock under in-order streams, and the
-model must reproduce the measured scaling of round 1 within 15 % (profiles/r01_bench_c4_{1,2,4,8}gpu.json)."""
+neither the default order nor the experimental AGP_DIST_SCHED=1 order may deadlock under in-order streams."""
 import importlib.util
-import json
 import os
 
 import pytest
@@ -20,11 +18,3 @@ def test_no_deadlock(R, sched2):
         pytest.skip("single rank uses cholesky_inplace")
     t = dsm.simulate(dsm.build(8192, R, 512, sched2, 16 if sched2 else 0, 0.7), R)
     assert t > 0
-
-
-def test_model_reproduces_measured_scaling():
-    for R in (1, 2, 4, 8):
-        with open(os.path.join(ROOT, "profiles", "r01_bench_c4_%dgpu.json" % R)) as f:
-            measured = json.load(f)["phases_ms"]["cholesky"]
-        model = dsm.simulate(dsm.build(65536, R, 512, False, 0, 1.0 if R == 1 else 0.7), R) * 1e3
-        assert abs(model / measured - 1.0) < 0.15, (R, model, measured)

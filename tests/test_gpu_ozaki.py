@@ -1,4 +1,4 @@
-"""tcgen05 int8-sliced (Ozaki) fp64 trailing update vs. a float64 reference computed with torch on the
+"""int8-sliced (Ozaki) fp64 trailing update (wgmma) vs. a float64 reference computed with torch on the
 same device (a floating-point kernel, so the reference is fp64 matmul; the exact-integer part of the
 scheme is additionally checked on integer-valued inputs, where the result must be bit-exact)."""
 import ctypes as C
@@ -69,7 +69,7 @@ def test_ozaki_persistent_lower_with_border(ag, N, K, S):
     assert np.array_equal(got[~low], c0[~low])
 
 
-# ---- generalised tcgen05 path (v3 kernel): fp32 / fp64 operands in either storage order, fp32 / fp64 output, rectangular
+# ---- generalised int8-slice path: fp32 / fp64 operands in either storage order, fp32 / fp64 output, rectangular
 # products with two operands in one slice workspace, accumulation sign -- the building block of the fp32 factorisation,
 # of the multi-RHS forward substitution (C.U' \ X, /root/reference/src/util/common_covmat_ops.jl:54,90) and of the VFE stream
 @pytest.mark.parametrize("M,N,K,S,cdt,adt,bdt,akm,bkm,sign", [

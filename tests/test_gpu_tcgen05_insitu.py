@@ -1,4 +1,4 @@
-"""The tcgen05 (int8-sliced, TMEM) factorisation checked IN PLACE: `agp_fit` driven through the path that runs every
+"""The int8-sliced tensor-core (wgmma) factorisation checked IN PLACE: `agp_fit` driven through the path that runs every
 n_pad >= 8192 fit (fp64_mode = 1, 512-wide outer panels, slicing, persistent trailing update, look-ahead) against the
 oracle -- logpdf rtol 1e-8 as BASELINE.json demands, alpha and the factor U -- plus the block-cyclic strip-table tile
 enumeration of the multi-GPU trailing update, driven on ONE device through `agp_debug_ozaki_syrk_map` exactly as
@@ -32,7 +32,7 @@ def forced_tcgen05(ag):
 
 @pytest.mark.parametrize("n", [1300, 2304, 4096])
 def test_fit_forced_tcgen05_matches_oracle(ag, forced_tcgen05, n):
-    """below the automatic threshold the engine is forced onto the tcgen05 path (the C2 workload at n = 4096)"""
+    """below the automatic threshold the engine is forced onto the int8-slice path (the C2 workload at n = 4096)"""
     eng = forced_tcgen05
     cfg = ref.make_config("C2", n=n)
     lp, post = _fit(ag, cfg)
@@ -44,7 +44,7 @@ def test_fit_forced_tcgen05_matches_oracle(ag, forced_tcgen05, n):
     assert np.isclose(post.data.C.logdet(), ref.logdet_chol(pr["U"]), rtol=1e-9)
     if n <= 2304:
         assert np.allclose(post.data.C.U, pr["U"], rtol=1e-7, atol=1e-9)
-    # the tcgen05 path really ran: its 2^-49 slice truncation makes it differ from the DMMA path in the last bits
+    # the int8-slice path really ran: its 2^-49 slice truncation makes it differ from the DMMA path in the last bits
     eng.set_config(fp64_mode=0, tile_nb=0)
     lp0, post0 = _fit(ag, cfg)
     eng.set_config(fp64_mode=1, tile_nb=512)
@@ -54,8 +54,8 @@ def test_fit_forced_tcgen05_matches_oracle(ag, forced_tcgen05, n):
 
 @pytest.mark.parametrize("n,d", [(8192, 16), (8320, 8), (16384, 8)])
 def test_fit_auto_mode_large_matches_oracle(ag, n, d):
-    """automatic policy (n_pad >= 8192 -> tcgen05, 512-wide panels): the path of every C4 number.  n = 8320 has a ragged
-    last outer panel (n_pad % 512 = 128): tcgen05 panels followed by a DMMA tail."""
+    """automatic policy (n_pad >= 8192 -> int8 slices, 512-wide panels): the path of every C4 number.  n = 8320 has a ragged
+    last outer panel (n_pad % 512 = 128): int8-slice panels followed by a DMMA tail."""
     cfg = ref.make_config("C4", n=n)
     cfg["X"] = np.ascontiguousarray(cfg["X"][:, :d])
     cfg["k"] = ref.KernelSpec(ref.SE, 1.0, ref.T_SCALE, scale=1.0 / (0.5 * np.sqrt(d)))
@@ -119,7 +119,7 @@ def test_strip_table_enumeration_matches_fp64(ag, R, me, kk, nto, W):
 # ---- fp32 on the tensor cores: the same int8-sliced kernel with 4 slices (28 bits cover the fp32 significand), fp32 C
 @pytest.mark.parametrize("n,d,fam", [(4224, 8, ref.SE), (6000, 32, ref.MATERN32)])
 def test_fp32_fit_on_tcgen05_matches_fp64_oracle(ag, n, d, fam):
-    """auto policy for fp32: n_pad >= 4096 -> 512-wide panels, tcgen05 trailing update; logpdf rtol 1e-4 (BASELINE.json)"""
+    """auto policy for fp32: n_pad >= 4096 -> 512-wide panels, int8-slice trailing update; logpdf rtol 1e-4 (BASELINE.json)"""
     cfg = ref.make_config("C3", n=n)
     X = np.ascontiguousarray(cfg["X"][:, :d])
     y = cfg["y"]
@@ -148,7 +148,7 @@ def test_fp32_fit_on_tcgen05_matches_fp64_oracle(ag, n, d, fam):
 
 def test_fp64_predict_uses_tensor_forward_substitution(ag):
     """mean_and_var at 1536 test points on an fp64 posterior with n_pad >= 2048: B[below] -= L[below, block] B[block] runs on
-    the tcgen05 kernel (7 slices, rectangular product); parity with the oracle at fp64 tolerances"""
+    the int8-slice kernel (7 slices, rectangular product); parity with the oracle at fp64 tolerances"""
     n, d = 3000, 6
     cfg = ref.make_config("C2", n=n)
     X = np.ascontiguousarray(cfg["X"][:, :d])

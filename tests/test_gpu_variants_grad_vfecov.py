@@ -1,15 +1,11 @@
-"""Variants of the tcgen05 trailing-update kernel, the device gradient of logpdf, the full covariance of the approximate
-posterior and the replays of the reference's own test sets.  All of this was written in round 1 without a GPU and first
-ran (green) on a B200 in round 2, call 1 (profiles/r02_call1.log); it is part of the default GPU suite since.  The kernel
-variants run in subprocesses under a timeout, so a protocol bug (the mbarrier spin limit traps) fails one test instead
-of poisoning the session.
+"""Variants of the int8-slice trailing-update kernel, the device gradient of logpdf, the full covariance of the approximate
+posterior and the replays of the reference's own test sets.  The kernel variants run in subprocesses under a timeout, so a
+protocol bug (the mbarrier spin limit traps) fails one test instead of poisoning the session.  Each must be bit-identical
+to the default launch (persistent grid, int32 pair pre-combination in the drain where K <= 512):
 
-* AGP_OZAKI_CLUSTER=2 -- 2-CTA clusters on one row tile, the A slices fetched half each and TMA-multicast;
-* AGP_OZAKI_EPIWARPS=4 -- one epilogue warp per TMEM lane quarter instead of two;
-  both must be bit-identical to the default kernel (umma_ozaki_syrk_v3_kernel<S, 1, 8, 0>);
-* AGP_OZAKI_CHUNK_TEST=4 -- bounded CTAs (4 consecutive tiles each) instead of the persistent grid of the debug entry.
-The round-1 kernel (v2) was removed in round 2 after v3 replaced it (profiles/r02_call2_ozaki_probe_v3.json keeps its last
-timings)."""
+* AGP_OZAKI_EPI=0 -- the plain int64 drain (the same exact integers, so the same single rounding);
+* AGP_OZAKI_CHUNK_TEST=1 / =4 -- bounded CTAs of 1 / 4 consecutive tiles each (the form the look-ahead schedule uses)
+  instead of the persistent grid of the debug entry."""
 import os
 import subprocess
 import sys
@@ -21,8 +17,8 @@ pytestmark = [pytest.mark.gpu]
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 
 
-@pytest.mark.parametrize("switches", [["AGP_OZAKI_CLUSTER=2"], ["AGP_OZAKI_EPIWARPS=4"],
-                                      ["AGP_OZAKI_CLUSTER=2", "AGP_OZAKI_EPIWARPS=4"], ["AGP_OZAKI_CHUNK_TEST=4"]])
+@pytest.mark.parametrize("switches", [["AGP_OZAKI_EPI=0"], ["AGP_OZAKI_CHUNK_TEST=1"],
+                                      ["AGP_OZAKI_EPI=0", "AGP_OZAKI_CHUNK_TEST=4"], ["AGP_OZAKI_CHUNK_TEST=4"]])
 @pytest.mark.parametrize("N,K,S", [(128, 128, 7), (1024, 256, 7), (4224, 512, 7), (2176, 512, 6), (8192, 512, 7), (1152, 1024, 8)])
 def test_variant_matches_default_kernel(N, K, S, switches):
     r = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "exp_variant_check.py"), str(N), str(K), str(S)] + switches,

@@ -1,6 +1,6 @@
-"""CPU model of the arithmetic of the tcgen05 int8-slice SYRK (abstractgps.jl_b200/csrc/umma_ozaki.cu): row-exponent
+"""CPU model of the arithmetic of the int8-slice SYRK (abstractgps.jl_b200/csrc/umma_ozaki.cu): row-exponent
 scaling, error-free 7-bit slicing (ozaki_slice_kernel), exact int32 accumulation per diagonal d = s + t (what the
-stacked-B MMAs leave in TMEM), and the two fp64 recombinations of the epilogue -- plain Horner (AGP_OZAKI_EPI=0) and the
+stacked-B MMAs leave in the accumulators), and the two fp64 recombinations of the epilogue -- plain Horner (AGP_OZAKI_EPI=0) and the
 int32 pair pre-combination that is the default for S = 7, K <= 512 (AGP_OZAKI_EPI=1).  Checks the bounds the kernel relies
 on: slices stay in [-64, 64], accumulators and pairs fit int32 for K <= 512 (and the pair does NOT fit at K = 1024, which is
 why the host falls back), both recombinations agree with exact integer arithmetic to fp64 rounding, and the final update
@@ -120,7 +120,7 @@ def test_umma_noswizzle_chunk_layout_halves():
     assert seen == set(range(4096))
 
 
-# ---- the v3 drain (round 2): exact int64 words + magic-number conversion + ONE rounding --------------------------------
+# ---- the drain: exact int64 words + magic-number conversion + ONE rounding --------------------------------
 MAGIC = 0x4338000000000000        # bit pattern of 2^52 + 2^51
 MAGIC_D = 6755399441055744.0      # 2^52 + 2^51
 
@@ -132,7 +132,7 @@ def i64_to_f64_exact(x):
 
 
 def oz_combine(acc, pair32):
-    """oz_combine<S, PAIR32> of csrc/umma_ozaki.cu on a [S, ...] int64 array of accumulators: value = sum_d acc_d 128^(3-d)"""
+    """oz_combine<S, BN, PAIR32> of csrc/umma_ozaki.cu on a [S, ...] int64 array of accumulators: value = sum_d acc_d 128^(3-d)"""
     S = acc.shape[0]
     a = acc.astype(np.int64)
     if S <= 4:
@@ -224,8 +224,9 @@ def test_fp32_operands_are_covered_by_short_splits(S, bits):
 def test_v3_slice_layout_matches_the_producer_addressing():
     """ozaki_slice_kernel (bulk == 2) writes byte (row, k, slice s) of the panel at
          chunk = ((row >> 7) * (K >> 5) + (k >> 5)) * S + s,   offset = chunk * 4096 + core-matrix offset(row & 127, k & 31);
-    the v3 producer fetches, for a 128-row tile at `arow` and k block kb, ONE run of S * 4096 bytes (A slices 0..S-1 in
-    order) and for a 64-row strip at `brow` S pieces of 2048 bytes at stride 4096 -- both must see exactly their rows."""
+    the producer fetches, for a 128-row tile at `arow` and k block kb, ONE run of S * 4096 bytes (A slices 0..S-1 in
+    order) and for a BN-row strip at `brow` (BN = 64 or 32) S pieces of BN * 32 bytes at stride 4096 -- both must see
+    exactly their rows."""
     S, K, rows = 7, 128, 512
     nkb = K >> 5
 
@@ -247,12 +248,12 @@ def test_v3_slice_layout_matches_the_producer_addressing():
             tile = a[sl * 4096:(sl + 1) * 4096]
             assert set(tile[:, 2]) == {sl} and set(tile[:, 0]) == set(range(arow, arow + 128))
             assert set(tile[:, 1]) == set(range(kb * 32, kb * 32 + 32))
-            # inside the tile: the UMMA no-swizzle K-major core-matrix layout (SBO 256 B, LBO 128 B)
+            # inside the tile: the no-swizzle K-major core-matrix layout of the MMA descriptors (SBO 256 B, LBO 128 B)
             r, k = 77, kb * 32 + 21
             assert tuple(tile[core(r, 21)]) == (arow + r, k, sl)
-    for brow, kb in ((0, 2), (64, 0), (192, 3), (448, 1)):
-        base = (brow >> 7) * rb_bytes + (brow & 64) * 32 + kb * S * 4096
+    for BN, brow, kb in ((64, 0, 2), (64, 64, 0), (64, 192, 3), (64, 448, 1), (32, 32, 1), (32, 96, 2), (32, 416, 0)):
+        base = (brow >> 7) * rb_bytes + (brow & 127) * 32 + kb * S * 4096
         for sl in range(S):
-            piece = buf[base + sl * 4096:][:2048]
-            assert set(piece[:, 2]) == {sl} and set(piece[:, 0]) == set(range(brow, brow + 64))
+            piece = buf[base + sl * 4096:][:BN * 32]
+            assert set(piece[:, 2]) == {sl} and set(piece[:, 0]) == set(range(brow, brow + BN))
             assert set(piece[:, 1]) == set(range(kb * 32, kb * 32 + 32))

@@ -1,6 +1,6 @@
 """Drive the DISTRIBUTED fit path on ONE GPU (a 1-rank NCCL communicator) in host-pointer and device-pointer mode and
-print the library's phase timings -- to see whether the e2e-only slowdown of the "gram" phase seen at 2 and 8 ranks
-(profiles/r02_call7_8gpu.log) is a property of the path or of several processes sharing a host.
+print the library's phase timings -- to see whether an e2e-only slowdown of the "gram" phase seen at several ranks
+is a property of the path or of several processes sharing a host.
 Usage: python tools/dist1_probe.py N D [reps]"""
 import ctypes as C
 import importlib.util

@@ -1,6 +1,6 @@
 """Discrete-event model of the distributed (block-column-cyclic) Cholesky schedule of fit_dist_impl
 (abstractgps.jl_b200/csrc/engine.cu): per rank two in-order streams, CUDA-event edges, one NCCL broadcast per outer panel,
-and the one hardware fact that shapes everything -- the persistent tcgen05 update kernel holds every SM it was launched
+and the one hardware fact that shapes everything -- the persistent int8-slice update kernel holds every SM it was launched
 on until it ends, so whatever is enqueued behind it (the next panel's factorisation, the NCCL kernel of the next
 broadcast) waits for it.
 
@@ -8,13 +8,13 @@ broadcast) waits for it.
 
 It replays the op order of the C++ loop for the default schedule and for AGP_DIST_SCHED=1 (owner defers its rest update
 behind the next panel's factorisation; updates leave `reserve` SMs to NCCL), checks that neither order can deadlock,
-and prints the modelled makespan.  Durations come from single-GPU measurements of this round (profiles/): update kernel
-60 TFLOP/s fp64-equivalent at full width x a narrow-update efficiency, panel factorisation = 0.28 ms of latency-bound
-chain + its flops at 20 TFLOP/s, broadcast at 350 GB/s.  The model is for ranking schedules, not for predicting ms."""
+and prints the modelled makespan.  Durations come from ASSUMED rates, not measurements: update kernel 60 TFLOP/s
+fp64-equivalent at full width x a narrow-update efficiency, panel factorisation = 0.28 ms of latency-bound chain + its
+flops at 20 TFLOP/s, broadcast at 350 GB/s.  The model is for ranking schedules, not for predicting ms."""
 import argparse
 import heapq
 
-NSM = 148
+NSM = 132  # H100 SXM
 
 
 class Op:
