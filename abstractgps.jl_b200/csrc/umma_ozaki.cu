@@ -15,10 +15,14 @@
 //
 // One kernel, ozaki_syrk_wgmma_kernel: persistent or bounded CTAs walking a list of 128 x BN output tiles; one producer
 // warp streams the slices with bulk copies, two consumer warpgroups (64 rows each) issue the MMAs and drain their own
-// accumulators.  For A slice s one wgmma runs against the STACK of B slices 0..S-1-s (consecutive in shared memory,
-// N = (S-s)*BN), so the products of diagonal d land in accumulator block d: S MMAs per 32-byte K chunk instead of
-// S(S+1)/2.  The S accumulator blocks of 64 x BN int32 live in registers (S*BN/2 per thread), which sets BN:
-// 64 for S <= 4, 32 above.
+// accumulators.  Per 32-byte K chunk a consumer loads each A slice's 64 x 32-byte fragment into registers once
+// (ldmatrix) and issues S(S+1)/2 uniform m64nBNk32 MMAs, one per slice pair (s, t), into accumulator block d = s + t;
+// only B is read from shared memory.  The blocks never overlap, so ptxas pipelines the issue; wider MMAs against a
+// stack of B slices would write overlapping accumulator fragments of different widths, which ptxas serialises.  The
+// fragments are double-buffered so one chunk's MMAs stay in flight while the next chunk's fragments load.  The S
+// accumulator blocks of 64 x BN int32 live in registers (S*BN/2 per thread), which sets BN: 64 for S <= 4, 32 above.
+// The producer also stages the tile's old C block into shared memory halfway through the tile's K loop, so the drain's
+// read-modify-write does not wait on HBM (partial or unaligned tiles read C from global memory as before).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -203,17 +207,28 @@ struct OzTileArgs {
   const int32_t* strip_bimin;    // table walk: first valid 128-row tile of every strip
   const int8_t* SL;              // slices in the blocked layout [128-row block][32-byte k chunk][slice][4096 B]
   int epi;                       // drain: 0 Horner-style int64 words, 1 int32 pair pre-combination (K <= 512)
+  int c_bulk;                    // C and ldc 16-byte aligned: full tiles stage their C block by bulk copies
 };
 
-// per slice count: output tile 128 x BN, pipeline depth
-template <int S>
+// per slice count and C type: output tile 128 x BN, pipeline depth, staged C block (column-major, every column padded
+// by 16 bytes so the drain's shared-memory reads are free of bank conflicts)
+template <int S, typename CT>
 struct OzCfg {
   static constexpr int BN = (S <= 4) ? 64 : 32;
   static constexpr int A_BYTES = OZ_BM * OZ_KC, B_BYTES = BN * OZ_KC;
   static constexpr int STAGE_BYTES = S * (A_BYTES + B_BYTES);
-  static constexpr int STAGES = (200 * 1024 / STAGE_BYTES) > 6 ? 6 : (200 * 1024 / STAGE_BYTES);
-  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + 1024;
+  static constexpr int C_LD = OZ_BM + 16 / (int)sizeof(CT);  // elements per staged C column
+  static constexpr int C_BYTES = BN * C_LD * (int)sizeof(CT);
+  static constexpr int RING = 220 * 1024 - C_BYTES;
+  static constexpr int STAGES = (RING / STAGE_BYTES) > 6 ? 6 : (RING / STAGE_BYTES);
+  static constexpr size_t SMEM = (size_t)STAGES * STAGE_BYTES + C_BYTES + 1024;
 };
+
+// a tile stages its C block when it lies inside C and the bulk copies are aligned; producer and consumers decide alike
+template <int BN>
+__device__ __forceinline__ bool oz_c_staged(const OzTileArgs& a, int bi, int bj) {
+  return a.c_bulk && (int64_t)(bi + 1) * OZ_BM <= a.M && (int64_t)(bj + 1) * BN <= a.N;
+}
 
 // slot index -> (bi, bj) for the diagonal-anchored lower triangle (R = 128 / BN column tiles per row tile), L2-BLOCKED:
 // the tile grid is cut into 2048 x 2048 super-blocks (SB row tiles x R*SB column tiles); slots walk one super-block at a
@@ -302,12 +317,57 @@ __device__ __forceinline__ double oz_combine(const uint32_t* acc, int i) {
   return fma(i64_to_f64_exact(l), LO_SCALE, i64_to_f64_exact(h));
 }
 
-// the S MMAs of one 32-byte K chunk: A slice s (64 rows) against the stack of B slices 0..S-1-s -> accumulator blocks s..S-1
-template <int S, int BN, int s>
-__device__ __forceinline__ void oz_issue(uint32_t* acc, uint64_t adesc, uint64_t bdesc, uint32_t acc_in) {
-  if constexpr (s < S) {
-    WgmmaI8<(S - s) * BN>::mma(acc + s * (BN / 2), adesc + (uint64_t)(s * (OZ_BM * OZ_KC >> 4)), bdesc, s == 0 ? acc_in : 1u);
-    oz_issue<S, BN, s + 1>(acc, adesc, bdesc, acc_in);
+__device__ __forceinline__ void ldsm_x4(uint32_t* r, uint32_t saddr) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]) : "r"(saddr) : "memory");
+}
+
+// one 32-byte K chunk of one consumer warpgroup.  sa: the stage; a_lane: this lane's ldmatrix row address inside a
+// 4096-byte A chunk (the four 8 x 16-byte core matrices of the warp's 16 rows are exactly the register fragment).
+// Loads the S A fragments, then issues A slice s against B slice t into accumulator block s + t for every s + t < S.
+// af must not belong to an MMA still in flight.
+template <int S, int BN>
+__device__ __forceinline__ void oz_chunk(uint32_t* acc, uint32_t (&af)[S][4], uint32_t sa, uint32_t a_lane, uint32_t acc_in) {
+  constexpr int A_BYTES = OZ_BM * OZ_KC, B_BYTES = BN * OZ_KC;
+#pragma unroll
+  for (int s = 0; s < S; ++s) ldsm_x4(af[s], sa + s * A_BYTES + a_lane);
+  const uint64_t bdesc = desc_nosw(sa + S * A_BYTES);
+  wgmma_fence();
+#pragma unroll
+  for (int s = 0; s < S; ++s)
+#pragma unroll
+    for (int t = 0; t < S - s; ++t)  // s = 0 writes every block first: acc_in = 0 starts the tile
+      WgmmaI8<BN>::mma(acc + (s + t) * (BN / 2), af[s], bdesc + (uint64_t)(t * (B_BYTES >> 4)), s == 0 ? acc_in : 1u);
+  wgmma_commit();
+}
+
+// the drain of one consumer thread: rows r0, r0 + 8 of the tile and columns 8j + 2(lane & 3) + {0, 1} of every
+// accumulator block; C += sign * (2^e_i 2^e_j 2^-33) * v with rs[h] = sign 2^e_i 2^-33, streamed (.cs) so the int8
+// slices stay resident in L2.  STAGED: a full tile whose old C is in the staged block; otherwise guarded global loads.
+template <int S, int BN, bool PAIR32, bool STAGED, typename CT>
+__device__ __forceinline__ void oz_drain(const OzTileArgs& a, const uint32_t* acc, const CT* cbuf, int bi, int bj, int64_t brow,
+                                         int r0, const double* rs) {
+  constexpr int C_LD = OzCfg<S, CT>::C_LD;
+  CT* C = (CT*)a.C;
+  const int64_t m0 = (int64_t)bi * OZ_BM + r0;
+  const int cq = 2 * ((threadIdx.x & 31) & 3);
+#pragma unroll
+  for (int i0 = 0; i0 < BN / 2; i0 += 8) {  // 8 elements (two 8-column groups) per round: loads first, then stores
+    double cv[8];
+#pragma unroll
+    for (int i = i0; i < i0 + 8; ++i) {
+      const int c = 8 * (i >> 2) + cq + (i & 1), h = (i >> 1) & 1;
+      const int64_t row = m0 + 8 * h, col = (int64_t)bj * BN + c;
+      if constexpr (STAGED) cv[i - i0] = (double)cbuf[c * C_LD + r0 + 8 * h];
+      else cv[i - i0] = (row < a.M && col < a.N) ? ld_cs(C + row + col * a.ldc) : 0.0;
+    }
+#pragma unroll
+    for (int i = i0; i < i0 + 8; ++i) {
+      const int c = 8 * (i >> 2) + cq + (i & 1), h = (i >> 1) & 1;
+      const int64_t row = m0 + 8 * h, col = (int64_t)bj * BN + c;
+      const double v = oz_combine<S, BN, PAIR32>(acc, i);
+      if (STAGED || (row < a.M && col < a.N)) st_cs(C + row + col * a.ldc, fma(v, rs[h] * a.rscale[brow + c], cv[i - i0]));
+    }
   }
 }
 
@@ -317,23 +377,27 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileA
   // [b * tpc, (b + 1) * tpc) and exits; the grid is ceil(ntiles / tpc).  Bounded CTAs hand their SM back every ~0.1 ms, so
   // kernels of a higher-priority stream (the panel chain, the NCCL broadcast) are scheduled between them instead of
   // waiting for the whole update.
-  using Cfg = OzCfg<S>;
+  using Cfg = OzCfg<S, CT>;
   constexpr int BN = Cfg::BN, STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
-  constexpr int A_BYTES = Cfg::A_BYTES, B_BYTES = Cfg::B_BYTES;
+  constexpr int A_BYTES = Cfg::A_BYTES, B_BYTES = Cfg::B_BYTES, C_LD = Cfg::C_LD;
   const int64_t t_begin = tpc ? (int64_t)blockIdx.x * tpc : (int64_t)blockIdx.x;
   const int64_t t_end = tpc ? ((t_begin + tpc < ntiles) ? t_begin + tpc : ntiles) : ntiles;
   const int64_t t_step = tpc ? 1 : (int64_t)gridDim.x;
   extern __shared__ __align__(1024) uint8_t smem[];
-  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES];
+  __shared__ __align__(8) uint64_t full_bar[STAGES], empty_bar[STAGES], c_full, c_empty;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   uint8_t* base = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem) + 1023) & ~(uintptr_t)1023);
+  CT* cbuf = reinterpret_cast<CT*>(base + STAGES * STAGE_BYTES);  // staged C block [BN][C_LD]
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < STAGES; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 8); }
+    mbar_init(&c_full, 1);
+    mbar_init(&c_empty, 8);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   __syncthreads();
-  const int num_kb = a.K / OZ_KC;
+  const int num_kb = a.K / OZ_KC;  // even: K % 64 == 0
+  uint32_t cn = 0;                 // staged C blocks so far (parity of c_full / c_empty)
 
   if (warp >= 8) {
     // the producer warpgroup hands its registers to the consumers (128 x 40 + 256 x 232 <= 64K)
@@ -350,7 +414,18 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileA
       const int64_t arow = (int64_t)bi * OZ_BM + a.a_off;
       const int8_t* asrc = a.SL + (arow >> 7) * rb_bytes;
       const int8_t* bsrc = a.SL + (brow >> 7) * rb_bytes + (brow & 127) * OZ_KC;
+      const bool staged = oz_c_staged<BN>(a, bi, bj);
       for (int kb = 0; kb < num_kb; ++kb, ++it) {
+        if (staged && kb == num_kb / 2) {
+          // the tile's C block, one bulk copy per column, half a tile ahead of the drain; by now the consumers are
+          // normally past the previous tile's drain, so the wait for the buffer does not stall the ring
+          mbar_wait(&c_empty, (cn & 1) ^ 1);
+          if (lane == 0) mbar_expect_tx(&c_full, BN * OZ_BM * (uint32_t)sizeof(CT));
+          __syncwarp();
+          const CT* csrc = (const CT*)a.C + (int64_t)bi * OZ_BM + (int64_t)bj * BN * a.ldc;
+          for (int c = lane; c < BN; c += 32) bulk_load(cbuf + c * C_LD, csrc + c * a.ldc, OZ_BM * sizeof(CT), &c_full);
+          ++cn;
+        }
         const uint32_t st = it % STAGES, ph = (it / STAGES) & 1;
         mbar_wait(&empty_bar[st], ph ^ 1);
         if (elect_one()) {
@@ -370,9 +445,14 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileA
     asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
     const int wg = warp >> 2;
     uint32_t acc[S * BN / 2];
+    // A fragments of the even / odd K chunks, so one chunk's MMAs stay in flight while the next chunk's fragments load;
+    // one buffer (and a full wait per chunk) where two would not fit next to the accumulators (S = 8)
+    constexpr int NAF = (S * BN / 2 + 2 * 4 * S <= 168) ? 2 : 1;
+    uint32_t af[NAF][S][4];
     uint32_t it = 0;
     const uint32_t smem0 = smem_u32(base);
-    const bool pair32 = (a.epi == 1);
+    // ldmatrix.x4 row address: lanes 8j .. 8j+7 read core matrix j = (row group 8 wg + 2 (warp & 3) + (j & 1), K half j >> 1)
+    const uint32_t a_lane = (((8 * wg + 2 * (warp & 3) + ((lane >> 3) & 1)) * 2 + (lane >> 4)) * 8 + (lane & 7)) * 16;
     for (int64_t t = t_begin; t < t_end; t += t_step) {
       int bi, bj;
       int64_t brow;
@@ -381,43 +461,45 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileA
         const uint32_t st = it % STAGES, ph = (it / STAGES) & 1;
         mbar_wait(&full_bar[st], ph);
         const uint32_t sa = smem0 + st * STAGE_BYTES;
-        wgmma_fence();
-        oz_issue<S, BN, 0>(acc, desc_nosw(sa + wg * (A_BYTES / 2)), desc_nosw(sa + S * A_BYTES), kb != 0 ? 1u : 0u);
-        wgmma_commit();
-        if (kb > 0) {  // the previous chunk's MMAs are done: its stage may be refilled
-          wgmma_wait<1>();
-          if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+        if constexpr (NAF == 2) {
+          // the fragments of chunk kb - 2 are free: its MMAs completed at the wait below in iteration kb - 1
+          if (kb & 1) oz_chunk<S, BN>(acc, af[NAF - 1], sa, a_lane, 1u);
+          else oz_chunk<S, BN>(acc, af[0], sa, a_lane, kb != 0 ? 1u : 0u);
+          if (kb > 0) {  // the previous chunk's MMAs are done: its stage may be refilled
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+          }
+        } else {
+          oz_chunk<S, BN>(acc, af[0], sa, a_lane, kb != 0 ? 1u : 0u);
+          wgmma_wait<0>();
+          if (lane == 0) mbar_arrive(&empty_bar[st]);
         }
       }
-      wgmma_wait<0>();
-      if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      if constexpr (NAF == 2) {
+        wgmma_wait<0>();
+        if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+      }
 
-      // drain: thread holds rows m0, m0 + 8 and columns 8j + 2(lane & 3) + {0, 1} of every accumulator block;
-      // C += sign * (2^e_i 2^e_j 2^-33) * v, streamed (.cs) so the int8 slices stay resident in L2
-      const int64_t m0 = (int64_t)bi * OZ_BM + 64 * wg + 16 * (warp & 3) + (lane >> 2);
-      const int cq = 2 * (lane & 3);
+      const int r0 = 64 * wg + 16 * (warp & 3) + (lane >> 2);  // row inside the tile
       double rs[2];
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        const int64_t row = m0 + 8 * h;
+        const int64_t row = (int64_t)bi * OZ_BM + r0 + 8 * h;
         rs[h] = row < a.M ? a.sign * a.rscale[row + a.a_off] * (1.0 / 8589934592.0) : 0.0;  // +-2^e_i * 2^-12 * 128^-3
       }
-      CT* C = (CT*)a.C;
-#pragma unroll
-      for (int i0 = 0; i0 < BN / 2; i0 += 8) {  // 8 elements (two 8-column groups) per round: loads first, then stores
-        double cv[8];
-#pragma unroll
-        for (int i = i0; i < i0 + 8; ++i) {
-          const int64_t row = m0 + 8 * ((i >> 1) & 1), col = (int64_t)bj * BN + 8 * (i >> 2) + cq + (i & 1);
-          cv[i - i0] = (row < a.M && col < a.N) ? ld_cs(C + row + col * a.ldc) : 0.0;
-        }
-#pragma unroll
-        for (int i = i0; i < i0 + 8; ++i) {
-          const int c = 8 * (i >> 2) + cq + (i & 1);
-          const int64_t row = m0 + 8 * ((i >> 1) & 1), col = (int64_t)bj * BN + c;
-          const double v = pair32 ? oz_combine<S, BN, true>(acc, i) : oz_combine<S, BN, false>(acc, i);
-          if (row < a.M && col < a.N) st_cs(C + row + col * a.ldc, fma(v, rs[(i >> 1) & 1] * a.rscale[brow + c], cv[i - i0]));
-        }
+      const bool staged = oz_c_staged<BN>(a, bi, bj);
+      if (staged) mbar_wait(&c_full, cn & 1);
+      if (a.epi == 1) {
+        if (staged) oz_drain<S, BN, true, true>(a, acc, cbuf, bi, bj, brow, r0, rs);
+        else oz_drain<S, BN, true, false>(a, acc, cbuf, bi, bj, brow, r0, rs);
+      } else {
+        if (staged) oz_drain<S, BN, false, true>(a, acc, cbuf, bi, bj, brow, r0, rs);
+        else oz_drain<S, BN, false, false>(a, acc, cbuf, bi, bj, brow, r0, rs);
+      }
+      if (staged) {  // this warp has read its part of the staged block
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&c_empty);
+        ++cn;
       }
     }
   }
@@ -428,7 +510,7 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileA
 template <int S, typename CT>
 int launch_syrk_wgmma(const OzakiWs& ws, void* C, int64_t ldc, int64_t M, int64_t N, int64_t b_tile_stride,
                       int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s, int full, double sign) {
-  using Cfg = OzCfg<S>;
+  using Cfg = OzCfg<S, CT>;
   constexpr int BN = Cfg::BN, R = OZ_BM / BN;
   static uint64_t configured = 0;  // per-device bit: the attribute is per device (one ctx per GPU in one process)
   static int nsm = 0;
@@ -443,6 +525,7 @@ int launch_syrk_wgmma(const OzakiWs& ws, void* C, int64_t ldc, int64_t M, int64_
   a.b_tile_stride = b_tile_stride; a.b_tile_width = b_tile_width; a.b_off = b_off; a.a_off = a_off;
   a.SL = ws.SL;
   a.sign = sign;
+  a.c_bulk = ((uintptr_t)C % 16 == 0) && ((uint64_t)ldc * sizeof(CT)) % 16 == 0;
   {
     // default: the int32 pair pre-combination (S >= 5, K <= 512: bit-identical to the int64 words, fewer integer ops);
     // AGP_OZAKI_EPI=0 restores the plain int64 drain
