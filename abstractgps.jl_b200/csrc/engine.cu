@@ -220,8 +220,7 @@ void trailing_update(agp_ctx* ctx, T* L, int64_t lda, int64_t row0, int64_t col0
   bool done = false;
   if (oz) {  // int8-sliced tensor-core path: the slices of panel rows [oz_row0, ...) are already in *oz
     if constexpr (std::is_same<T, double>::value) {
-      ozaki_syrk(*oz, L + row0 + col0 * lda, lda, M, N, 1, 0, 0, col0 - oz_row0, row0 - oz_row0, st);
-      done = true;
+      done = ozaki_syrk(*oz, L + row0 + col0 * lda, lda, M, N, 1, 0, 0, col0 - oz_row0, row0 - oz_row0, st) == 0;
     } else {
       done = ozaki_update_ex(*oz, L + row0 + col0 * lda, 1, lda, M, N, 0, -1.0, 0, 0, col0 - oz_row0, row0 - oz_row0, st) == 0;
     }
@@ -1870,7 +1869,7 @@ int fit_dist_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
     if (ctx->profile) cudaEventRecord(prof_event(ctx), st);
     bool done = false;
     if constexpr (std::is_same<T, double>::value) {
-      if (use_oz) { ozaki_syrk(*oz_cur, C, lda, rows_below, Ncols, 1, (int64_t)R * W, W, b_off, 0, st); done = true; }
+      if (use_oz) done = ozaki_syrk(*oz_cur, C, lda, rows_below, Ncols, 1, (int64_t)R * W, W, b_off, 0, st) == 0;
     }
     if (!done) {
       GemmArgs u{};
@@ -2358,16 +2357,20 @@ int32_t agp_rand(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mea
 int32_t agp_debug_ozaki_syrk(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* P_dev, int64_t lda, int64_t M, int64_t N,
                              int32_t K, int32_t S, int32_t lower_only) {
   if (!ctx || !C_dev || !P_dev) return AGP_ERR_INVALID;
+  // the N columns pair with panel rows 0 .. N-1, so they must be among the M rows that are sliced
+  if (M <= 0 || N <= 0 || N > M || ldc < M) { ctx->err = "ozaki syrk: need 0 < N <= M <= ldc"; return AGP_ERR_INVALID; }
+  if (S < 5 || S > 8) { ctx->err = "ozaki syrk: fp64 C takes 5..8 slices"; return AGP_ERR_UNSUPPORTED; }
   cudaSetDevice(ctx->device);
   OzakiWs ws;
   int rc = ozaki_ws_create(&ws, M, K, S, ctx->stream);
   if (rc) { ctx->err = "ozaki_ws_create failed (code " + std::to_string(rc) + ")"; return rc == 1 ? AGP_ERR_INVALID : AGP_ERR_CUDA; }
   ozaki_prepare(ws, (const double*)P_dev, lda, M, ctx->stream);
-  ozaki_syrk(ws, (double*)C_dev, ldc, M, N, lower_only, 0, 0, 0, 0, ctx->stream);
+  const int urc = ozaki_syrk(ws, (double*)C_dev, ldc, M, N, lower_only, 0, 0, 0, 0, ctx->stream);
   ozaki_ws_destroy(&ws, ctx->stream);
   cudaError_t e = cudaStreamSynchronize(ctx->stream);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { ctx->err = std::string("ozaki syrk: ") + cudaGetErrorString(e); return AGP_ERR_CUDA; }
+  if (urc) { ctx->err = "ozaki syrk: slice count or strip table not supported"; return AGP_ERR_UNSUPPORTED; }
   return AGP_OK;
 }
 
@@ -2378,6 +2381,8 @@ int32_t agp_debug_ozaki_gemm(agp_ctx* ctx, void* C_dev, int32_t c_is_float, int6
                              int32_t a_kmajor, int64_t lda, int64_t M, const void* B_dev, int32_t b_is_float, int32_t b_kmajor,
                              int64_t ldb, int64_t N, int32_t K, int32_t S, double sign) {
   if (!ctx || !C_dev || !A_dev) return AGP_ERR_INVALID;
+  // without B the N columns pair with rows 0 .. N-1 of A, so they must be among its M sliced rows
+  if (M <= 0 || N <= 0 || ldc < M || (!B_dev && N > M)) { ctx->err = "ozaki gemm: need 0 < M <= ldc, 0 < N (N <= M without B)"; return AGP_ERR_INVALID; }
   cudaSetDevice(ctx->device);
   const int64_t m_pad = (M + 127) / 128 * 128, n_rows = B_dev ? (N + 127) / 128 * 128 : 0;
   OzakiWs ws;
@@ -2402,16 +2407,26 @@ int32_t agp_debug_ozaki_syrk_map(agp_ctx* ctx, void* C_dev, int64_t ldc, const v
                                  int64_t b_off, int64_t a_off) {
   if (!ctx || !C_dev || !P_dev) return AGP_ERR_INVALID;
   if (N % 128 != 0 || N < 128 || M <= 0 || m_panel <= 0) { ctx->err = "N must be a positive multiple of 128"; return AGP_ERR_INVALID; }
+  // rows and columns address the sliced panel in whole 128-row blocks: offsets and the column map must stay inside it
+  const int64_t bw = b_tile_width ? b_tile_width : 128;
+  const int64_t last_col_row = (b_tile_stride ? ((N - 1) / bw) * b_tile_stride + (N - 1) % bw : N - 1) + b_off;
+  if (a_off < 0 || b_off < 0 || a_off % 128 || b_off % 128 || b_tile_stride % 128 || bw % 128 || ldc < M ||
+      M + a_off > m_panel || last_col_row >= m_panel) {
+    ctx->err = "ozaki syrk (map): rows or columns outside the panel (offsets, stride and width in multiples of 128)";
+    return AGP_ERR_INVALID;
+  }
+  if (S < 5 || S > 8) { ctx->err = "ozaki syrk (map): fp64 C takes 5..8 slices"; return AGP_ERR_UNSUPPORTED; }
   cudaSetDevice(ctx->device);
   OzakiWs ws;
   int rc = ozaki_ws_create(&ws, m_panel, K, S, ctx->stream);
   if (rc) { ctx->err = "ozaki_ws_create failed (code " + std::to_string(rc) + ")"; return rc == 1 ? AGP_ERR_INVALID : AGP_ERR_CUDA; }
   ozaki_prepare(ws, (const double*)P_dev, lda, m_panel, ctx->stream);
-  ozaki_syrk(ws, (double*)C_dev, ldc, M, N, 1, b_tile_stride, b_tile_width, b_off, a_off, ctx->stream);
+  const int urc = ozaki_syrk(ws, (double*)C_dev, ldc, M, N, 1, b_tile_stride, b_tile_width, b_off, a_off, ctx->stream);
   ozaki_ws_destroy(&ws, ctx->stream);
   cudaError_t e = cudaStreamSynchronize(ctx->stream);
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { ctx->err = std::string("ozaki syrk (map): ") + cudaGetErrorString(e); return AGP_ERR_CUDA; }
+  if (urc) { ctx->err = "ozaki syrk (map): strip table not supported"; return AGP_ERR_UNSUPPORTED; }
   return AGP_OK;
 }
 

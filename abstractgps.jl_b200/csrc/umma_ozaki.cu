@@ -25,6 +25,7 @@
 // read-modify-write does not wait on HBM (partial or unaligned tiles read C from global memory as before).
 #include <cuda.h>
 #include <cuda_runtime.h>
+#include <math_constants.h>
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -44,6 +45,9 @@ constexpr int OZ_THREADS = 384;         // warpgroups 0, 1: consumers; warpgroup
 // ---------------------------------------------------------------------------------------------
 // pre-pass 1: row exponents
 // ---------------------------------------------------------------------------------------------
+// |x| for the row maximum, with NaN mapped to +inf: fmax would drop a NaN and the row would lose it silently
+__device__ __forceinline__ double oz_mag(double x) { return isnan(x) ? CUDART_INF : fabs(x); }
+
 template <typename Tin>
 __global__ void __launch_bounds__(256) ozaki_rowscale_kernel(const Tin* __restrict__ P, int64_t lda, int64_t m, int K, int kmajor,
                                                              double* __restrict__ rscale, double* __restrict__ rinv) {
@@ -58,7 +62,7 @@ __global__ void __launch_bounds__(256) ozaki_rowscale_kernel(const Tin* __restri
     if (row < m) {
       const Tin* p = P + row + (int64_t)y * lda;
 #pragma unroll 4
-      for (int k = y; k < K; k += 8, p += 8 * lda) mx = fmax(mx, fabs((double)*p));
+      for (int k = y; k < K; k += 8, p += 8 * lda) mx = fmax(mx, oz_mag((double)*p));
     }
     part[y][x] = mx;
     __syncthreads();
@@ -71,7 +75,7 @@ __global__ void __launch_bounds__(256) ozaki_rowscale_kernel(const Tin* __restri
       const int64_t r2 = blockIdx.x * 32ll + rr;
       double v = 0.0;
       if (r2 < m)
-        for (int k = lane; k < K; k += 32) v = fmax(v, fabs((double)P[k + r2 * lda]));
+        for (int k = lane; k < K; k += 32) v = fmax(v, oz_mag((double)P[k + r2 * lda]));
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) v = fmax(v, __shfl_xor_sync(0xffffffffu, v, o));
       if (lane == 0) part[0][rr] = v;
@@ -84,8 +88,11 @@ __global__ void __launch_bounds__(256) ozaki_rowscale_kernel(const Tin* __restri
   if (row < m) {
     int e = 0;
     if (mx > 0.0 && isfinite(mx)) frexp(mx, &e);  // mx = f * 2^e, f in [0.5, 1)
-    rscale[row] = ldexp(1.0, e);
-    rinv[row] = ldexp(1.0, -e);
+    if (e < -1022) e = -1022;  // subnormal rows: 2^1022 scales them exactly and keeps rinv finite
+    // a NaN or +-Inf entry, or a maximum >= 2^1023 (2^e overflows): every output the row touches becomes NaN
+    const bool bad = !(mx < 0x1p1023);
+    rscale[row] = bad ? CUDART_NAN : ldexp(1.0, e);
+    rinv[row] = bad ? 0.0 : ldexp(1.0, -e);
   }
 }
 
@@ -114,7 +121,8 @@ __global__ void ozaki_slice_kernel(const Tin* __restrict__ P, int64_t lda, int64
     union { int8_t b[16]; uint4 v; } pk;
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
-      const double q = rint(r[i] * up);
+      double q = rint(r[i] * up);
+      if (!(fabs(q) <= 64.0)) q = 0.0;  // only a non-finite entry gets here (its row scale is NaN): no int conversion of it
       r[i] = fma(-q, dn, r[i]);
       pk.b[i] = (int8_t)(int)q;
     }
@@ -658,14 +666,15 @@ int ozaki_update_ex(const OzakiWs& ws, void* C, int c_is_float, int64_t ldc, int
 #undef AGP_UPD
 }
 
-void ozaki_syrk(const OzakiWs& ws, double* C, int64_t ldc, int64_t M, int64_t N, int lower_only, int64_t b_tile_stride,
-                int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s) {
-  if (M <= 0 || N <= 0) return;
+int ozaki_syrk(const OzakiWs& ws, double* C, int64_t ldc, int64_t M, int64_t N, int lower_only, int64_t b_tile_stride,
+               int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s) {
+  if (M <= 0 || N <= 0) return 0;
   const int full = lower_only ? 0 : 1;
   switch (ws.S) {
-    case 5: launch_syrk_wgmma<5, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0); break;
-    case 6: launch_syrk_wgmma<6, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0); break;
-    case 7: launch_syrk_wgmma<7, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0); break;
-    default: launch_syrk_wgmma<8, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0); break;
+    case 5: return launch_syrk_wgmma<5, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    case 6: return launch_syrk_wgmma<6, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    case 7: return launch_syrk_wgmma<7, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    case 8: return launch_syrk_wgmma<8, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    default: return 1;  // fp64 C is instantiated for 5..8 slices only (a 3- or 4-slice workspace is for fp32 panels)
   }
 }

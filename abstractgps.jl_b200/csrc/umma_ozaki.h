@@ -27,9 +27,10 @@ void ozaki_ws_destroy(OzakiWs* ws, cudaStream_t s);
 void ozaki_prepare(const OzakiWs& ws, const double* P, int64_t lda, int64_t m, cudaStream_t s);
 // C (M x N, ldc) -= P P'  using the slices in ws; column n of C pairs with panel row
 // (n/128)*b_tile_stride + n%128 + b_off  (b_tile_stride = 0: n + b_off), row r of C with panel row r + a_off;
-// lower_only skips tiles above the diagonal
-void ozaki_syrk(const OzakiWs& ws, double* C, int64_t ldc, int64_t M, int64_t N, int lower_only, int64_t b_tile_stride,
-                int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s);
+// lower_only skips tiles above the diagonal.  Returns 0 once launched, 1 (nothing launched) if ws.S is not 5..8 or the
+// strip table of the shape does not fit the workspace; the caller must then run the update another way.
+int ozaki_syrk(const OzakiWs& ws, double* C, int64_t ldc, int64_t M, int64_t N, int lower_only, int64_t b_tile_stride,
+               int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s);
 
 // generalised entry points:
 //  * operands may be fp32 or fp64, row-contiguous (element (row, k) at P[row + k*lda]) or k-major (P[k + row*lda]); the
