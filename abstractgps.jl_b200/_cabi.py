@@ -18,9 +18,24 @@ AGP_MEM_HOST, AGP_MEM_DEVICE = 0, 1
  AGP_ERR_INVALID) = range(7)
 
 
+AGP_RQ, AGP_PERIODIC, AGP_WHITE, AGP_CONSTANT, AGP_COMPOSITE = 5, 6, 7, 8, 9
+AGP_COMPOSITE_MAX = 8  # terms, and factors in all
+
+
+class agp_kernel_factor(C.Structure):
+    _fields_ = [("family", C.c_int32), ("transform", C.c_int32), ("scale", C.c_double), ("param", C.c_double),
+                ("ard", C.c_void_p), ("r", C.c_void_p)]
+
+
+class agp_kernel_composite(C.Structure):
+    _fields_ = [("nterms", C.c_int32), ("nfactors", C.POINTER(C.c_int32)), ("variance", C.POINTER(C.c_double)),
+                ("factors", C.POINTER(agp_kernel_factor))]
+
+
 class agp_kernel(C.Structure):
     _fields_ = [("family", C.c_int32), ("transform", C.c_int32), ("variance", C.c_double),
-                ("scale", C.c_double), ("linear_c", C.c_double), ("ard", C.c_void_p)]
+                ("scale", C.c_double), ("linear_c", C.c_double), ("ard", C.c_void_p),
+                ("composite", C.POINTER(agp_kernel_composite))]
 
 
 class agp_mean(C.Structure):
@@ -62,6 +77,7 @@ SIGNATURES = {
     "agp_post_logpdf": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _M, _N, _P, C.c_int32, _P]),
     "agp_post_rand": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _M, _N, _P, C.c_int32, _P]),
     "agp_post_logpdf_grad": (C.c_int32, [_P, C.POINTER(C.c_double), _P]),
+    "agp_post_grad_len": (C.c_int64, [_P]),
     "agp_post_solve_lower": (C.c_int32, [_P, _P, C.c_int64, _P]),
     "agp_post_factor_export": (C.c_int32, [_P, _P]),
     "agp_post_logdet": (C.c_int32, [_P, C.POINTER(C.c_double)]),

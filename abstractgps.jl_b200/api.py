@@ -22,6 +22,7 @@ from ._cabi import AGPError, DimensionMismatch, PosDefException  # noqa: F401
 # KernelFunctions.jl surface that AbstractGPs re-exports (src/AbstractGPs.jl:8)
 # ---------------------------------------------------------------------------------------------
 SE, MATERN12, MATERN32, MATERN52, LINEAR = range(5)
+RQ, PERIODIC, WHITE, CONSTANT = cabi.AGP_RQ, cabi.AGP_PERIODIC, cabi.AGP_WHITE, cabi.AGP_CONSTANT
 
 
 class Transform:
@@ -39,20 +40,38 @@ class ARDTransform(Transform):
 
 
 class Kernel:
-    """sigma_f^2 * (kappa o transform) -- the kernel set the engine implements on device."""
+    """sigma_f^2 * (kappa o transform) -- the kernel set the engine implements on device.  RationalQuadratic (alpha),
+    Periodic (r), White and Constant (c) are valid only inside a sum or product (KernelSum / KernelProduct)."""
 
-    def __init__(self, family, variance=1.0, transform: Optional[Transform] = None, c=0.0):
+    def __init__(self, family, variance=1.0, transform: Optional[Transform] = None, c=0.0, alpha=2.0, r=None,
+                 scaled=False):
         self.family, self.variance, self.transform, self.c = family, float(variance), transform, float(c)
+        self.alpha = float(alpha)
+        self.r = None if r is None else np.ascontiguousarray(r, dtype=np.float64).ravel()
+        self.scaled = scaled  # built as sigma^2 * k: sigma^2 is a parameter of the tree (kernel_params)
+
+    def _copy(self, variance=None, transform=None, scaled=None):
+        return Kernel(self.family, self.variance if variance is None else variance,
+                      self.transform if transform is None else transform, self.c, self.alpha, self.r,
+                      self.scaled if scaled is None else scaled)
 
     def __rmul__(self, s):  # sigma^2 * k  (ScaledKernel)
-        return Kernel(self.family, self.variance * float(s), self.transform, self.c)
+        return self._copy(variance=self.variance * float(s), scaled=True)
 
-    __mul__ = __rmul__
+    def __mul__(self, o):  # k1 * k2 (KernelProduct); k * sigma^2 (ScaledKernel)
+        if isinstance(o, Kernel):
+            return KernelProduct(self, o)
+        return self.__rmul__(o)
+
+    def __add__(self, o):  # k1 + k2 (KernelSum)
+        if not isinstance(o, Kernel):
+            return NotImplemented
+        return KernelSum(self, o)
 
     def compose(self, t: Transform):  # k o t  (TransformedKernel)
         if self.transform is not None:
             t = _chain(self.transform, t)
-        return Kernel(self.family, self.variance, t, self.c)
+        return self._copy(transform=t)
 
     __matmul__ = compose
 
@@ -62,7 +81,7 @@ class Kernel:
     def _key(self):
         t = self.transform
         tk = None if t is None else (("s", t.s) if isinstance(t, ScaleTransform) else ("a", tuple(t.v)))
-        return (self.family, self.variance, tk, self.c)
+        return (self.family, self.variance, tk, self.c, self.alpha, None if self.r is None else tuple(self.r))
 
     __hash__ = None
 
@@ -115,6 +134,268 @@ def with_lengthscale(k: Kernel, ell):
     if np.ndim(ell) == 0:
         return k.compose(ScaleTransform(1.0 / float(ell)))
     return k.compose(ARDTransform(1.0 / np.asarray(ell, dtype=np.float64)))
+
+
+def RationalQuadraticKernel(alpha: float = 2.0):
+    """(1 + d^2 / (2 alpha))^(-alpha); a factor of a composite kernel."""
+    return Kernel(RQ, alpha=alpha)
+
+
+def PeriodicKernel(r=(1.0,)):
+    """exp(-1/2 sum_i (sinpi(x_i - y_i) / r_i)^2); a factor of a composite kernel.  A length-1 r applies to every
+    dimension."""
+    return Kernel(PERIODIC, r=r)
+
+
+def WhiteKernel():
+    """1 if the (transformed) inputs are equal, else 0; a factor of a composite kernel."""
+    return Kernel(WHITE)
+
+
+def ConstantKernel(c: float = 1.0):
+    """c; a factor of a composite kernel."""
+    return Kernel(CONSTANT, c=c)
+
+
+class _CompositeKernel(Kernel):
+    """A sum or product of kernels, itself optionally scaled (sigma^2 * k) and transformed (k o t).  Scaling or
+    transforming it applies to every leaf, as in KernelFunctions; flattening (_Flat) carries that out."""
+
+    def __init__(self, *kernels, variance=1.0, transform=None, scaled=False):
+        self.kernels = []
+        for k in kernels:  # (k1 + k2) + k3 is one sum of three, like KernelFunctions' KernelSum
+            if type(k) is type(self) and not k.scaled and k.transform is None:
+                self.kernels.extend(k.kernels)
+            else:
+                self.kernels.append(k)
+        self.family, self.variance, self.transform, self.scaled = cabi.AGP_COMPOSITE, float(variance), transform, scaled
+        self.c, self.alpha, self.r = 0.0, 2.0, None
+
+    def _copy(self, variance=None, transform=None, scaled=None):
+        out = type(self).__new__(type(self))
+        out.__dict__.update(self.__dict__)
+        out.kernels = list(self.kernels)
+        if variance is not None:
+            out.variance = variance
+        if transform is not None:
+            out.transform = transform
+        if scaled is not None:
+            out.scaled = scaled
+        return out
+
+    def _key(self):
+        t = self.transform
+        tk = None if t is None else (("s", t.s) if isinstance(t, ScaleTransform) else ("a", tuple(t.v)))
+        return (type(self).__name__, self.variance, tk, tuple(k._key() for k in self.kernels))
+
+
+class KernelSum(_CompositeKernel):
+    """k1 + k2 + ..."""
+
+
+class KernelProduct(_CompositeKernel):
+    """k1 * k2 * ..."""
+
+
+def _walk(k: Kernel, vals: list):
+    """Depth-first: register k's parameters in `vals` (scaling, transform, then the family's own) and return its terms:
+    [(scaling parameter indices, [factor, ...])], a factor being a dict with its family and the indices of its
+    transforms (innermost first), parameter and r."""
+    sc = []
+    if k.scaled or k.variance != 1.0:  # Kernel(family, variance=v) carries its variance like a ScaledKernel
+        vals.append(k.variance)
+        sc = [len(vals) - 1]
+    tr = []
+    if k.transform is not None:
+        t = k.transform
+        vals.append(t.s if isinstance(t, ScaleTransform) else np.array(t.v, dtype=np.float64))
+        tr = [len(vals) - 1]
+    if isinstance(k, KernelSum):
+        terms = [tm for ch in k.kernels for tm in _walk(ch, vals)]
+    elif isinstance(k, KernelProduct):
+        terms = [([], [])]
+        for ch in k.kernels:  # a product over a sum is distributed
+            ct = _walk(ch, vals)
+            terms = [(a[0] + b[0], a[1] + b[1]) for a in terms for b in ct]
+    else:
+        f = dict(family=k.family, tr=[], p=None, r=None)
+        if k.family == RQ:
+            vals.append(k.alpha)
+            f["p"] = len(vals) - 1
+        elif k.family in (LINEAR, CONSTANT):
+            vals.append(k.c)
+            f["p"] = len(vals) - 1
+        if k.family == PERIODIC:
+            vals.append(np.array(k.r if k.r is not None else [1.0], dtype=np.float64))
+            f["r"] = len(vals) - 1
+        terms = [([], [f])]
+    return [(sc + s_, [dict(f, tr=f["tr"] + tr) for f in fs]) for s_, fs in terms]
+
+
+def _prod_except(vals, idx, skip, D=None):
+    """prod of vals[i] for i in idx except position `skip` (no division by a parameter); vectors broadcast to D"""
+    out = 1.0 if D is None else np.ones(D)
+    for j, i in enumerate(idx):
+        if j != skip:
+            out = out * (vals[i] if D is None or np.ndim(vals[i]) == 0 else np.broadcast_to(vals[i], (D,)))
+    return out
+
+
+class _Flat:
+    """A kernel tree flattened into the engine's sum of product terms, with what the chain rule needs to map the
+    descriptor's gradient back onto kernel_params(k)."""
+
+    def __init__(self, k: Kernel, D: int):
+        self.vals = []
+        self.terms = _walk(k, self.vals)
+        self.D = D
+        nf = sum(len(fs) for _, fs in self.terms)
+        if len(self.terms) > cabi.AGP_COMPOSITE_MAX or nf > cabi.AGP_COMPOSITE_MAX:
+            raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "composite kernel flattens to %d terms and %d factors; the device "
+                           "takes at most %d of each" % (len(self.terms), nf, cabi.AGP_COMPOSITE_MAX))
+        for _, fs in self.terms:
+            for f in fs:
+                for i in f["tr"] + ([f["r"]] if f["r"] is not None else []):
+                    if np.ndim(self.vals[i]) and self.vals[i].shape[0] not in (1, D):
+                        raise DimensionMismatch("a per-dimension kernel parameter has length %d, inputs have D=%d"
+                                                % (self.vals[i].shape[0], D))
+
+    def transform_of(self, f):
+        """(AGP_T_*, s, v) of factor f: its transform chain multiplied out"""
+        if not f["tr"]:
+            return 0, 1.0, None
+        if all(np.ndim(self.vals[i]) == 0 for i in f["tr"]):
+            return 1, float(np.prod([self.vals[i] for i in f["tr"]])), None
+        return 2, 1.0, _prod_except(self.vals, f["tr"], -1, self.D)
+
+    def struct(self, dt, keep):
+        nt = len(self.terms)
+        facs = [f for _, fs in self.terms for f in fs]
+        nfa = (C.c_int32 * nt)(*[len(fs) for _, fs in self.terms])
+        var = (C.c_double * nt)(*[float(_prod_except(self.vals, s_, -1)) for s_, _ in self.terms])
+        fa = (cabi.agp_kernel_factor * len(facs))()
+        for j, f in enumerate(facs):
+            kind, s, v = self.transform_of(f)
+            fa[j].family, fa[j].transform, fa[j].scale = f["family"], kind, s
+            fa[j].param = float(self.vals[f["p"]]) if f["p"] is not None else 0.0
+            if v is not None:
+                a = np.ascontiguousarray(v, dtype=dt)
+                keep.append(a)
+                fa[j].ard = a.ctypes.data
+            if f["r"] is not None:
+                a = np.ascontiguousarray(np.broadcast_to(self.vals[f["r"]], (self.D,)), dtype=dt)
+                keep.append(a)
+                fa[j].r = a.ctypes.data
+        comp = cabi.agp_kernel_composite()
+        comp.nterms, comp.nfactors, comp.variance = nt, nfa, var
+        comp.factors = C.cast(fa, C.POINTER(cabi.agp_kernel_factor))
+        keep.extend([nfa, var, fa, comp])
+        ks = cabi.agp_kernel()
+        ks.family, ks.transform, ks.variance, ks.scale = cabi.AGP_COMPOSITE, 0, 1.0, 1.0
+        ks.composite = C.pointer(comp)
+        return ks
+
+    def grad_len(self):
+        n = 5
+        for _, fs in self.terms:
+            n += 1
+            for f in fs:
+                kind = self.transform_of(f)[0]
+                n += 1 if kind == 1 else (self.D if kind == 2 else 0)
+                n += 1 if f["p"] is not None else 0
+                n += self.D if f["r"] is not None else 0
+        return n
+
+    def params_grad(self, g):
+        """chain rule from the descriptor gradient g (agp_post_logpdf_grad layout) to kernel_params order: every copy that
+        flattening made of a parameter contributes; no division by a parameter's value"""
+        D = self.D
+        out = [np.zeros_like(np.asarray(v, dtype=np.float64)) if np.ndim(v) else 0.0 for v in self.vals]
+
+        def add(i, x):
+            if np.ndim(self.vals[i]) == 0:
+                out[i] = out[i] + float(np.sum(x))
+            elif self.vals[i].shape[0] == 1 and D > 1:
+                out[i] = out[i] + np.array([np.sum(x)])
+            else:
+                out[i] = out[i] + x
+        pos = 5
+        for s_, fs in self.terms:
+            for j, i in enumerate(s_):
+                add(i, g[pos] * _prod_except(self.vals, s_, j))
+            pos += 1
+            for f in fs:
+                kind = self.transform_of(f)[0]
+                if kind == 1:
+                    for j, i in enumerate(f["tr"]):
+                        add(i, g[pos] * _prod_except(self.vals, f["tr"], j))
+                    pos += 1
+                elif kind == 2:
+                    gv = np.asarray(g[pos:pos + D])
+                    for j, i in enumerate(f["tr"]):
+                        add(i, gv * _prod_except(self.vals, f["tr"], j, D))
+                    pos += D
+                if f["p"] is not None:
+                    add(f["p"], g[pos])
+                    pos += 1
+                if f["r"] is not None:
+                    add(f["r"], np.asarray(g[pos:pos + D]))
+                    pos += D
+        return out
+
+
+def _composite_diag(k: Kernel, a):
+    """kernelmatrix_diag of a composite kernel: sum_t v_t prod_f kappa_f(x, x) -- 1 for stationary, RQ, Periodic and
+    White factors, c for Constant, |x~|^2 + c for Linear (like the single-kernel Linear diagonal, formed host-side)"""
+    fl = _Flat(k, a.shape[1])
+    out = np.zeros(a.shape[0], dtype=a.dtype)
+    for s_, fs in fl.terms:
+        t = np.full(a.shape[0], _prod_except(fl.vals, s_, -1), dtype=a.dtype)
+        for f in fs:
+            if f["family"] == CONSTANT:
+                t = t * a.dtype.type(fl.vals[f["p"]])
+            elif f["family"] == LINEAR:
+                kind, s, v = fl.transform_of(f)
+                xt = a * (a.dtype.type(s) if v is None else v.astype(a.dtype))
+                t = t * ((xt * xt).sum(1) + a.dtype.type(fl.vals[f["p"]]))
+        out = out + t
+    return out
+
+
+def kernel_params(k: Kernel):
+    """Depth-first list of every parameter of a kernel tree: each ScaledKernel sigma^2 (or variance other than 1), each
+    transform's s / v, and RQ
+    alpha, Periodic r, Linear c and Constant c -- the order of logpdf_grad(...)["kernel"] for a composite kernel."""
+    vals = []
+    _walk(k, vals)
+    return vals
+
+
+def with_kernel_params(k: Kernel, vals):
+    """The same tree with its parameters replaced, in kernel_params(k) order."""
+    it = iter(list(vals))
+
+    def rebuild(k):
+        variance = float(next(it)) if (k.scaled or k.variance != 1.0) else k.variance
+        t = k.transform
+        if t is not None:
+            v = next(it)
+            t = ScaleTransform(float(v)) if isinstance(t, ScaleTransform) else ARDTransform(v)
+        if isinstance(k, _CompositeKernel):
+            out = k._copy(variance=variance)
+            out.transform = t
+            out.kernels = [rebuild(ch) for ch in k.kernels]
+            return out
+        out = k._copy(variance=variance)
+        out.transform = t
+        if k.family == RQ:
+            out.alpha = float(next(it))
+        elif k.family in (LINEAR, CONSTANT):
+            out.c = float(next(it))
+        if k.family == PERIODIC:
+            out.r = np.ascontiguousarray(next(it), dtype=np.float64).ravel()
+        return out
+    return rebuild(k)
 
 
 class ColVecs:
@@ -281,7 +562,11 @@ def engine() -> Engine:
     return _engine
 
 
-def _kernel_struct(k: Kernel, dt, keep):
+def _kernel_struct(k: Kernel, dt, keep, D=None):
+    if isinstance(k, _CompositeKernel) or k.family > LINEAR:
+        if not isinstance(k, _CompositeKernel):  # a lone RQ / Periodic / White / Constant is a one-factor composite
+            k = KernelSum(k)
+        return _Flat(k, D).struct(dt, keep)
     ks = cabi.agp_kernel()
     ks.family, ks.variance, ks.linear_c, ks.scale = k.family, k.variance, k.c, 1.0
     t = k.transform
@@ -514,7 +799,7 @@ def _fit(fx: FiniteGP, Y, want_post: bool, want_alpha: bool):
         raise DimensionMismatch("length(fx) = %d but Y has %d rows" % (pts.n, Yf.shape[0]))
     S = Yf.shape[1]
     keep = []
-    ks = _kernel_struct(f.kernel, dt, keep)
+    ks = _kernel_struct(f.kernel, dt, keep, D=pts.D)
     ms = _mean_struct(f.mean.spec(pts, dt), keep)
     ns = _noise_struct(fx.s2, pts.n, dt, keep)
     lp = np.empty(S, dtype=dt)
@@ -619,18 +904,23 @@ def logpdf_grad(fx: FiniteGP, y):
     f = post.prior
     dt = post.data.C.dtype
     D = post.data.x.D
-    g = np.zeros(5 + D, dtype=np.float64)
+    k = f.kernel
+    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
+    g = np.zeros(int(eng.L.agp_post_grad_len(post.data.C.h)) if composite else 5 + D, dtype=np.float64)
     per_point = np.ndim(fx.s2) != 0
     nd = np.empty(len(fx), dtype=dt) if (per_point or isinstance(f.mean, CustomMean)) else None
     eng.check(eng.L.agp_post_logpdf_grad(post.data.C.h, g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd)))
-    k = f.kernel
-    out = {"variance": g[0]}
-    if isinstance(k.transform, ScaleTransform):
-        out["scale"] = g[1]
-    elif isinstance(k.transform, ARDTransform):
-        out["ard"] = g[5:5 + D].copy()
-    if k.family == LINEAR:
-        out["linear_c"] = g[2]
+    if composite:
+        # composite: out["kernel"][i] is the derivative in kernel_params(k)[i] (the descriptor's gradient mapped back)
+        out = {"kernel": _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D).params_grad(g)}
+    else:
+        out = {"variance": g[0]}
+        if isinstance(k.transform, ScaleTransform):
+            out["scale"] = g[1]
+        elif isinstance(k.transform, ARDTransform):
+            out["ard"] = g[5:5 + D].copy()
+        if k.family == LINEAR:
+            out["linear_c"] = g[2]
     out["noise"] = nd.astype(np.float64) if per_point else g[3]
     if isinstance(f.mean, ConstMean):
         out["mean_c"] = g[4]
@@ -666,7 +956,7 @@ def _gram(f: GP, pts: _Points, pts2: Optional[_Points], s2, dt):
     eng = engine()
     keep = []
     pts = pts.astype(dt)
-    ks = _kernel_struct(f.kernel, dt, keep)
+    ks = _kernel_struct(f.kernel, dt, keep, D=pts.D)
     ns = _noise_struct(s2, pts.n, dt, keep) if s2 is not None else None
     if pts2 is None:
         K = np.empty((pts.n, pts.n), dtype=dt, order="F")
@@ -763,6 +1053,8 @@ def var(f, x=None):
     if isinstance(f, GP):
         dt = np.result_type(pts.a.dtype, np.float32)
         k = f.kernel
+        if isinstance(k, _CompositeKernel) or k.family > LINEAR:
+            return _composite_diag(k if isinstance(k, _CompositeKernel) else KernelSum(k), pts.a.astype(dt))
         if k.family != LINEAR:
             return np.full(pts.n, k.variance, dtype=dt)
         a = pts.a.astype(dt)
@@ -848,7 +1140,7 @@ def rand_from_normals(fx: FiniteGP, Z, squeeze=False):
     pts = fx.x.astype(dt)
     Z = np.asfortranarray(np.asarray(Z, dtype=dt).reshape(pts.n, -1))
     keep = []
-    ks = _kernel_struct(f.kernel, dt, keep)
+    ks = _kernel_struct(f.kernel, dt, keep, D=pts.D)
     ms = _mean_struct(f.mean.spec(pts, dt), keep)
     ns = _noise_struct(fx.s2, pts.n, dt, keep)
     out = np.empty_like(Z, order="F")
@@ -927,7 +1219,7 @@ def _vfe_args(vfe: VFE, fx: FiniteGP, y):
         raise DimensionMismatch("the dimension of the projected GP (here: %d) must equal the number of targets "
                                 "(here: %d)" % (pts.n, y.shape[0]))
     keep = [y]
-    ks = _kernel_struct(f.kernel, dt, keep)
+    ks = _kernel_struct(f.kernel, dt, keep, D=pts.D)
     ms = _mean_struct(f.mean.spec(pts, dt), keep)
     ns = _noise_struct(fx.s2, pts.n, dt, keep)
     js = _noise_struct(vfe.fz.s2, z.n, dt, keep)

@@ -54,6 +54,15 @@ struct agp_ctx {
   int oz_S32 = 4;          // slices of the fp32 operands (4 x 7 bits >= the 24-bit significand)
 };
 
+// deep copy of an agp_kernel_composite: the launch descriptor (CompositeDesc, passed by value to the kernels) and the
+// per-accumulator weights, on the host (`w`, doubles) and on the device (`desc.w`, in the call's element type)
+struct CompState {
+  CompositeDesc desc{};
+  std::vector<double> w;   // 2 * nacc * D: weights, then 1/r, per accumulator
+  int64_t grad_len = 5;
+  bool owns_w = false;     // desc.w belongs to this state (a handle's copy) rather than to a call's scratch
+};
+
 struct agp_post {
   agp_ctx* ctx = nullptr;
   int dtype = AGP_F64;
@@ -78,6 +87,7 @@ struct agp_post {
   int64_t dist_W = 0;
   void* Lloc = nullptr;
   void* Dinv_loc = nullptr;
+  CompState* comp = nullptr;  // AGP_COMPOSITE: the handle's own descriptor (k.composite is not kept)
 };
 
 struct agp_vfe_post {
@@ -168,11 +178,125 @@ int download(agp_ctx* ctx, void* dst, const T* src, size_t count, bool always_ho
 
 int check_kernel(agp_ctx* ctx, const agp_kernel* k, int D) {
   if (!k) { ctx->err = "kernel spec is NULL"; return AGP_ERR_INVALID; }
+  if (k->family == AGP_COMPOSITE) {  // the descriptor itself is checked by comp_build
+    if (ctx->nccl) { ctx->err = "composite kernels are supported on a single-GPU context only"; return AGP_ERR_UNSUPPORTED; }
+    // the points are prepared with the top-level transform before the descriptor is read: reject it here, before any
+    // upload or launch (a composite carries its transforms in its factors)
+    if (k->transform != AGP_T_NONE || k->variance != 1.0) {
+      ctx->err = "a composite kernel takes transform AGP_T_NONE and variance 1 (scalings belong to the terms)";
+      return AGP_ERR_INVALID;
+    }
+    if (D <= 0) { ctx->err = "D must be positive"; return AGP_ERR_DIM_MISMATCH; }
+    return AGP_OK;
+  }
   if (k->family < AGP_SE || k->family > AGP_LINEAR) { ctx->err = "unsupported kernel family"; return AGP_ERR_UNSUPPORTED; }
   if (k->transform < AGP_T_NONE || k->transform > AGP_T_ARD) { ctx->err = "unsupported transform"; return AGP_ERR_UNSUPPORTED; }
   if (k->transform == AGP_T_ARD && !k->ard) { ctx->err = "ARD transform without weights"; return AGP_ERR_INVALID; }
   if (D <= 0) { ctx->err = "D must be positive"; return AGP_ERR_DIM_MISMATCH; }
   return AGP_OK;
+}
+
+// Validate an AGP_COMPOSITE kernel and flatten it into a CompState (host side; T = the call's element type, used to read
+// the ARD and r arrays).  Accumulators: every stationary / RQ / White factor with no transform or a Scale transform shares
+// ONE raw squared distance (d2 = s^2 raw), every such Linear factor one raw dot product; each ARD factor and each Periodic
+// factor has its own weighted sum.  Gradient slots follow the layout documented at agp_post_logpdf_grad.
+template <typename T>
+int comp_build(agp_ctx* ctx, const agp_kernel* k, int D, CompState* cs) {
+  const agp_kernel_composite* c = k->composite;
+  if (!c || !c->nfactors || !c->variance || !c->factors) { ctx->err = "composite kernel without its descriptor"; return AGP_ERR_INVALID; }
+  if (k->transform != AGP_T_NONE || k->variance != 1.0) {
+    ctx->err = "a composite kernel takes transform AGP_T_NONE and variance 1 (scalings belong to the terms)";
+    return AGP_ERR_INVALID;
+  }
+  if (c->nterms < 1 || c->nterms > AGP_COMP_MAX) { ctx->err = "composite kernel: 1..8 terms"; return AGP_ERR_INVALID; }
+  int nf = 0;
+  for (int t = 0; t < c->nterms; ++t) {
+    if (c->nfactors[t] < 1) { ctx->err = "composite kernel: every term needs at least one factor"; return AGP_ERR_INVALID; }
+    nf += c->nfactors[t];
+    if (nf > AGP_COMP_MAX) { ctx->err = "composite kernel: at most 8 factors in all"; return AGP_ERR_INVALID; }
+  }
+  CompositeDesc& d = cs->desc;
+  d = CompositeDesc{};
+  d.nterms = c->nterms;
+  d.nfactors = nf;
+  cs->w.clear();
+  int raw_sq = -1, raw_dot = -1;
+  auto new_acc = [&](int kind) {
+    const int a = d.nacc++;
+    d.acc_kind[a] = kind;
+    cs->w.resize((size_t)2 * d.nacc * D, 0.0);
+    for (int i = 0; i < D; ++i) cs->w[(size_t)2 * a * D + i] = 1.0;
+    return a;
+  };
+  int64_t slot = 5;
+  int f = 0;
+  for (int t = 0; t < c->nterms; ++t) {
+    d.variance[t] = c->variance[t];
+    d.g_var[t] = (int)slot++;
+    for (int j = 0; j < c->nfactors[t]; ++j, ++f) {
+      const agp_kernel_factor& in = c->factors[f];
+      CompFactor& F = d.f[f];
+      F.family = in.family; F.transform = in.transform; F.term = t;
+      F.s = in.transform == AGP_T_SCALE ? in.scale : 1.0;
+      F.s2 = 1.0; F.param = in.param;
+      F.g_s = F.g_p = F.g_w = F.g_r = -1;
+      if (in.family < AGP_SE || in.family > AGP_CONSTANT) { ctx->err = "composite kernel: unsupported factor family"; return AGP_ERR_UNSUPPORTED; }
+      if (in.transform < AGP_T_NONE || in.transform > AGP_T_ARD) { ctx->err = "composite kernel: unsupported factor transform"; return AGP_ERR_UNSUPPORTED; }
+      if (in.transform == AGP_T_ARD && !in.ard) { ctx->err = "composite kernel: ARD factor without weights"; return AGP_ERR_INVALID; }
+      if (in.family == AGP_RQ && !(in.param > 0.0)) { ctx->err = "composite kernel: RationalQuadratic alpha must be > 0"; return AGP_ERR_INVALID; }
+      const T* ard = (const T*)in.ard;
+      if (in.family == AGP_CONSTANT) {
+        F.acc = -1;
+      } else if (in.family == AGP_PERIODIC) {
+        F.acc = new_acc(COMP_ACC_PER);
+        for (int i = 0; i < D; ++i) {
+          const double r = in.r ? (double)((const T*)in.r)[i] : 1.0;
+          if (!(r > 0.0)) { ctx->err = "composite kernel: Periodic r must be > 0"; return AGP_ERR_INVALID; }
+          cs->w[(size_t)2 * F.acc * D + i] = in.transform == AGP_T_ARD ? (double)ard[i] : F.s;
+          cs->w[(size_t)(2 * F.acc + 1) * D + i] = 1.0 / r;
+        }
+      } else if (in.transform == AGP_T_ARD) {
+        F.acc = new_acc(in.family == AGP_LINEAR ? COMP_ACC_DOT : COMP_ACC_SQ);
+        for (int i = 0; i < D; ++i) cs->w[(size_t)2 * F.acc * D + i] = (double)ard[i];
+      } else if (in.family == AGP_LINEAR) {
+        if (raw_dot < 0) raw_dot = new_acc(COMP_ACC_DOT);
+        F.acc = raw_dot;
+        F.s2 = F.s * F.s;
+      } else {
+        if (raw_sq < 0) raw_sq = new_acc(COMP_ACC_SQ);
+        F.acc = raw_sq;
+        F.s2 = F.s * F.s;
+      }
+      if (in.transform == AGP_T_SCALE) F.g_s = (int)slot++;
+      else if (in.transform == AGP_T_ARD) { F.g_w = (int)slot; slot += D; }
+      if (in.family == AGP_RQ || in.family == AGP_LINEAR || in.family == AGP_CONSTANT) F.g_p = (int)slot++;
+      if (in.family == AGP_PERIODIC) { F.g_r = (int)slot; slot += D; }
+    }
+  }
+  if (d.nacc == 0) new_acc(COMP_ACC_SQ);  // Constant factors only: the kernels still carry one (unused) accumulator
+  cs->grad_len = slot;
+  return AGP_OK;
+}
+
+// the descriptor's weights on the device in the element type T: in the call's scratch, or owned by the state (handles)
+template <typename T>
+int comp_upload(agp_ctx* ctx, Scratch& sc, CompState* cs, bool own) {
+  std::vector<T> h(cs->w.begin(), cs->w.end());
+  void* dv = nullptr;
+  const size_t bytes = h.size() * sizeof(T);
+  if (own) CK(cudaMallocAsync(&dv, bytes, ctx->stream));
+  else CK(sc.alloc(&dv, bytes));
+  CK(cudaMemcpyAsync(dv, h.data(), bytes, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));  // h is a local
+  cs->desc.w = dv;
+  cs->owns_w = own;
+  return AGP_OK;
+}
+
+void comp_free(CompState* cs, cudaStream_t s) {
+  if (!cs) return;
+  if (cs->owns_w && cs->desc.w) cudaFreeAsync((void*)cs->desc.w, s);
+  delete cs;
 }
 
 void prof_begin(agp_ctx* ctx) { ctx->prof_used = 0; }
@@ -517,7 +641,8 @@ void forward_subst_multi(agp_ctx* ctx, const T* L, int64_t lda, const T* Dinv, i
 
 template <typename T>
 void fill_gram_params(GramParams& gp, const agp_kernel* k, int symmetric, int lower_only, int64_t va, int64_t vb,
-                      const agp_noise* noise, const T* noise_v_dev) {
+                      const agp_noise* noise, const T* noise_v_dev, const CompState* comp = nullptr) {
+  gp.comp = comp ? &comp->desc : nullptr;
   gp.family = k->family;
   gp.variance = k->variance;
   gp.linear_c = k->linear_c;
@@ -562,6 +687,9 @@ int fit_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
   if (mean->kind == 2 && !mean->v) { ctx->err = "mean vector is NULL"; return AGP_ERR_INVALID; }
   if (noise->kind == 1 && !noise->v) { ctx->err = "noise vector is NULL"; return AGP_ERR_INVALID; }
 
+  CompState comp_local;
+  if (k->family == AGP_COMPOSITE) { rc = comp_build<T>(ctx, k, D, &comp_local); if (rc) return rc; }
+
   cudaStream_t s = ctx->stream;
   CK(cudaSetDevice(ctx->device));
   Scratch sc(ctx);
@@ -585,6 +713,13 @@ int fit_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
   const bool keep = (post_out != nullptr);
   rc = prep_points<T>(ctx, sc, k, ard_d, layout, X, N, n_pad, D, &Xt, keep);
   if (rc) return rc;
+  CompState* comp = nullptr;
+  if (k->family == AGP_COMPOSITE) {
+    comp = keep ? new CompState(comp_local) : &comp_local;
+    rc = comp_upload<T>(ctx, sc, comp, keep);
+    if (rc) { if (keep) comp_free(comp, s); return rc; }
+  }
+  struct CompGuard { CompState* c; cudaStream_t s; ~CompGuard() { if (c) comp_free(c, s); } } cguard{keep ? comp : nullptr, s};
   CK(cudaEventRecord(ctx->ev[1], s));
 
   // ---- buffers
@@ -601,7 +736,9 @@ int fit_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
     post->ctx = ctx; post->dtype = sizeof(T) == 8 ? AGP_F64 : AGP_F32;
     post->n = N; post->n_pad = n_pad; post->lda = lda; post->D = D;
     post->L = Lv; post->Dinv = Dinvv; post->Xt = Xt; post->alpha = alphav;
-    post->k = *k; post->k.ard = nullptr;
+    post->k = *k; post->k.ard = nullptr; post->k.composite = nullptr;
+    post->comp = comp;  // freed with the handle
+    cguard.c = nullptr;
     post->mean_kind = mean->kind == 2 ? 0 : mean->kind; post->mean_c = mean->c;
     post->segs.push_back({0, N});
     CK(cudaMallocAsync(&post->delta, (size_t)n_pad * sizeof(T), s));
@@ -631,7 +768,7 @@ int fit_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
 
   // ---- Gram (+ noise) straight into the factor buffer, border rows = delta'
   GramParams gp{};
-  fill_gram_params<T>(gp, k, 1, 1, N, N, noise, noise_d);
+  fill_gram_params<T>(gp, k, 1, 1, N, N, noise, noise_d, comp);
   launch_gram<T>(Xt, Xt, n_pad, n_pad, D, L, lda, gp, s);
   launch_border_init<T>(L, lda, N, n_pad, Yd, N, S, mean->kind, mean->c, mean_d, s);
   if (keep) {
@@ -757,7 +894,7 @@ int post_cross(agp_post* p, Scratch& sc, int layout, const void* Xs, int64_t M, 
   CK(sc.alloc(&b, (size_t)p->n_pad * m_pad * sizeof(T)));
   *B = (T*)b;
   GramParams gp{};
-  fill_gram_params<T>(gp, &p->k, 0, 0, p->n, M, nullptr, nullptr);
+  fill_gram_params<T>(gp, &p->k, 0, 0, p->n, M, nullptr, nullptr, p->comp);
   gp.mask_a = p->valid;
   launch_gram<T>((const T*)p->Xt, *Xst, p->n_pad, m_pad, p->D, *B, p->n_pad, gp, ctx->stream);
   return AGP_OK;
@@ -808,7 +945,7 @@ int post_mean_var_impl(agp_post* p, int layout, const void* Xs, int64_t M, const
     void* tmp = nullptr;
     CK(sc.alloc(&tmp, (size_t)m_pad * 3 * sizeof(T)));
     T* mu = (T*)tmp; T* var = mu + m_pad; T* kd = var + m_pad;
-    launch_kdiag<T>(Xst, mc, p->D, p->k.family, p->k.variance, p->k.linear_c, kd, s);
+    launch_kdiag<T>(Xst, mc, p->D, p->k.family, p->k.variance, p->k.linear_c, kd, s, p->comp ? &p->comp->desc : nullptr);
     launch_gemv_t<T>(B, p->n_pad, p->n_pad, mc, (const T*)p->alpha, mean_s->kind, mean_s->c, mean_d, mu, s);
     if (var_out) {
       forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, p->n_pad, B, p->n_pad, m_pad);
@@ -937,7 +1074,7 @@ int post_mean_cov_impl(agp_post* p, int layout, const void* Xs, int64_t M, const
     g.C = C; g.ldc = m_pad; g.M = m_pad; g.N = m_pad; g.K = p->n_pad;
     launch_gemm<T>(g, s);
     GramParams gp{};
-    fill_gram_params<T>(gp, &p->k, 1, 0, M, M, nullptr, nullptr);
+    fill_gram_params<T>(gp, &p->k, 1, 0, M, M, nullptr, nullptr, p->comp);
     launch_gram<T>(Xst, Xst, m_pad, m_pad, p->D, Kss, m_pad, gp, s);
     launch_cov_finish<T>(C, m_pad, Kss, m_pad, s);
     cudaMemcpyKind kind = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
@@ -996,7 +1133,7 @@ int post_cond_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp
   CK(sc.alloc(&tmp, (size_t)nblk * TILE * TILE * sizeof(T)));
   T* Dinv = (T*)tmp;
   GramParams gp{};
-  fill_gram_params<T>(gp, &p->k, 1, 1, M, M, noise_s, noise_d);
+  fill_gram_params<T>(gp, &p->k, 1, 1, M, M, noise_s, noise_d, p->comp);
   launch_gram<T>(Xst, Xst, m_pad, m_pad, p->D, Lf, ldf, gp, s);
   {
     GemmArgs g{};
@@ -1073,12 +1210,13 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out) {
   T* V = (T*)tmp;
   CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
   T* Cinv = (T*)tmp;
-  CK(sc.alloc(&tmp, (size_t)(5 + D) * sizeof(double)));
+  const int64_t nsums = agp_post_grad_len(p);  // 5 + D for a single kernel
+  CK(sc.alloc(&tmp, (size_t)nsums * sizeof(double)));
   double* sums = (double*)tmp;
   T* noise_d = nullptr;
   if (noise_diag_out) { CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T))); noise_d = (T*)tmp; }
   CK(cudaMemsetAsync(V, 0, (size_t)n_pad * n_pad * sizeof(T), s));
-  CK(cudaMemsetAsync(sums, 0, (size_t)(5 + D) * sizeof(double), s));
+  CK(cudaMemsetAsync(sums, 0, (size_t)nsums * sizeof(double), s));
   launch_add_diag<T>(V, n_pad, n_pad, 1.0, s);
   forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, V, n_pad, n_pad);
   {
@@ -1087,6 +1225,18 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out) {
     g.B = V; g.ldb = n_pad; g.b_kmajor = 1;
     g.C = Cinv; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = 1;
     launch_gemm<T>(g, s);
+  }
+  if (p->comp) {  // composite: every kernel slot is 1/2 sum_ij W_ij dK_ij/dtheta, already in its final place
+    launch_composite_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->comp->desc, sums, noise_d, s);
+    std::vector<double> h((size_t)nsums);
+    CK(cudaMemcpyAsync(h.data(), sums, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (noise_diag_out) { int rc = download<T>(ctx, noise_diag_out, noise_d, (size_t)n, false); if (rc) return rc; }
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    for (int64_t i = 0; i < nsums; ++i) grad_out[i] = 0.5 * h[(size_t)i];
+    grad_out[0] = grad_out[1] = grad_out[2] = 0.0;
+    grad_out[4] = h[4];
+    return AGP_OK;
   }
   const int want_ard = (p->k.transform == AGP_T_ARD) ? 1 : 0;
   launch_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->k.family, p->k.linear_c, want_ard,
@@ -1226,11 +1376,11 @@ int post_extend_impl(agp_post* p, int layout, const void* X2, int64_t N2, const 
   launch_sub_mean<T>(y2d, N2, mean2->kind, mean2->c, mean_d, (T*)dn + n1p, s);
   // C21 = K(x2, x1) and C22 = K(x2, x2) + Sigma_y2 straight into the new factor buffer
   GramParams g21{};
-  fill_gram_params<T>(g21, &p->k, 0, 0, N2, p->n, nullptr, nullptr);
+  fill_gram_params<T>(g21, &p->k, 0, 0, N2, p->n, nullptr, nullptr, p->comp);
   g21.mask_b = valid;  // old rows (first n1p entries of the new mask)
   launch_gram<T>(X2t, (const T*)Xn, n2p, n1p, D, L + n1p, ldn, g21, s);
   GramParams g22{};
-  fill_gram_params<T>(g22, &p->k, 1, 1, N2, N2, noise2, noise_d);
+  fill_gram_params<T>(g22, &p->k, 1, 1, N2, N2, noise2, noise_d, p->comp);
   launch_gram<T>(X2t, X2t, n2p, n2p, D, L + n1p + n1p * ldn, ldn, g22, s);
   launch_border_init<T>(L, ldn, np, np, (const T*)dn, np, 1, 0, 0.0, (const T*)nullptr, s);
   // panel solves of the new rows (+ border) against the old factor
@@ -1291,6 +1441,15 @@ int post_extend_impl(agp_post* p, int layout, const void* X2, int64_t N2, const 
     if (p->ard) {
       cudaMallocAsync(&q->ard, (size_t)D * sizeof(T), s);
       cudaMemcpyAsync(q->ard, p->ard, (size_t)D * sizeof(T), cudaMemcpyDeviceToDevice, s);
+    }
+    if (p->comp) {  // the new handle owns its own copy of the descriptor
+      q->comp = new CompState(*p->comp);
+      const size_t wb = p->comp->w.size() * sizeof(T);
+      void* wd = nullptr;
+      cudaMallocAsync(&wd, wb, s);
+      cudaMemcpyAsync(wd, p->comp->desc.w, wb, cudaMemcpyDeviceToDevice, s);
+      q->comp->desc.w = wd;
+      q->comp->owns_w = true;
     }
     *post_out = q;
     p = q;
@@ -1357,6 +1516,8 @@ int gram_impl(agp_ctx* ctx, const agp_kernel* k, int layout, const void* X, int6
   if (N <= 0 || (Z && M <= 0)) { ctx->err = "empty input"; return AGP_ERR_DIM_MISMATCH; }
   cudaStream_t s = ctx->stream;
   CK(cudaSetDevice(ctx->device));
+  CompState comp_local, *comp = nullptr;
+  if (k->family == AGP_COMPOSITE) { rc = comp_build<T>(ctx, k, D, &comp_local); if (rc) return rc; comp = &comp_local; }
   Scratch sc(ctx);
   const int64_t n_pad = round_up(N, 64);
   const int64_t cols = Z ? M : N, c_pad = round_up(cols, 64);
@@ -1366,10 +1527,11 @@ int gram_impl(agp_ctx* ctx, const agp_kernel* k, int layout, const void* X, int6
   rc = prep_points<T>(ctx, sc, k, ard_d, layout, X, N, n_pad, D, &Xt, false);
   if (rc) return rc;
   if (Z) { rc = prep_points<T>(ctx, sc, k, ard_d, layout, Z, M, c_pad, D, &Zt, false); if (rc) return rc; }
+  if (comp) { rc = comp_upload<T>(ctx, sc, comp, false); if (rc) return rc; }
   void* tmp = nullptr;
   CK(sc.alloc(&tmp, (size_t)n_pad * c_pad * sizeof(T)));
   GramParams gp{};
-  fill_gram_params<T>(gp, k, Z ? 0 : 1, 0, N, cols, Z ? nullptr : noise, noise_d);
+  fill_gram_params<T>(gp, k, Z ? 0 : 1, 0, N, cols, Z ? nullptr : noise, noise_d, comp);
   launch_gram<T>(Xt, Z ? Zt : Xt, n_pad, c_pad, D, (T*)tmp, n_pad, gp, s);
   cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   CK(cudaMemcpy2DAsync(K_out, (size_t)N * sizeof(T), tmp, (size_t)n_pad * sizeof(T), (size_t)N * sizeof(T), (size_t)cols, kout, s));
@@ -1390,6 +1552,10 @@ template <typename T>
 int vfe_core(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout,
              const void* X, int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y,
              void* elbo_out, void* dtc_out, agp_vfe_post** post_out) {
+  if (k && k->family == AGP_COMPOSITE) {
+    ctx->err = "composite kernels are supported on the exact path only (not VFE)";
+    return AGP_ERR_UNSUPPORTED;
+  }
   int rc = check_kernel(ctx, k, D);
   if (rc) return rc;
   if (N <= 0 || M <= 0) { ctx->err = "N and M must be positive"; return AGP_ERR_DIM_MISMATCH; }
@@ -2343,8 +2509,14 @@ int32_t agp_post_free(agp_post* p) {
   if (p->valid) cudaFreeAsync(p->valid, s);
   if (p->Lloc) cudaFreeAsync(p->Lloc, s);
   if (p->Dinv_loc) cudaFreeAsync(p->Dinv_loc, s);
+  comp_free(p->comp, s);
   delete p;
   return AGP_OK;
+}
+
+int64_t agp_post_grad_len(const agp_post* p) {
+  if (!p) return 0;
+  return p->comp ? p->comp->grad_len : 5 + (int64_t)p->D;
 }
 
 int32_t agp_rand(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,

@@ -17,6 +17,7 @@
 // sums[5 + d] = sum w q tdiff_d^2  |  sum w tx_d tx'_d  (linear)        (-> d/d ard_d)
 #include "kernels.h"
 #include "agp.h"
+#include "composite.cuh"
 
 namespace {
 
@@ -192,7 +193,336 @@ grad_reduce_kernel(const T* __restrict__ Xt, int D, int64_t n, const T* __restri
   }
 }
 
+// ---- composite kernels ---------------------------------------------------------------------------------------------
+// kappa_f from its accumulator value x and, in fp64: ds = d kappa / d s (Scale transform on a shared raw accumulator),
+// dp = d kappa / d param (RQ alpha, Linear / Constant c), q = 2 d kappa / d d2 (stationary / RQ: the ARD pass uses
+// q v_d diff_d^2), or kappa itself for a Periodic factor (its pass needs kappa sin_d^2 / r_d^3 and the sinpi cospi terms)
+__device__ __forceinline__ void comp_factor_grad(const CompFactor& F, double x, double& kap, double& ds, double& dp,
+                                                 double& q) {
+  const double d2 = x * F.s2;
+  ds = 0.0; dp = 0.0; q = 0.0;
+  switch (F.family) {
+    case AGP_SE: { const double e = exp(-0.5 * d2); kap = e; q = -e; break; }
+    case AGP_MATERN12: { const double d = sqrt(d2), e = exp(-d); kap = e; q = d > 0.0 ? -e / d : 0.0; break; }
+    case AGP_MATERN32: {
+      const double s = 1.7320508075688772935 * sqrt(d2), e = exp(-s);
+      kap = (1.0 + s) * e; q = -3.0 * e;
+      break;
+    }
+    case AGP_MATERN52: {
+      const double s = 2.2360679774997896964 * sqrt(d2), e = exp(-s);
+      kap = (1.0 + s + s * s * (1.0 / 3.0)) * e; q = -(5.0 / 3.0) * (1.0 + s) * e;
+      break;
+    }
+    case AGP_RQ: {
+      const double a = F.param, u = d2 / (2.0 * a);
+      kap = pow(1.0 + u, -a);
+      q = -kap / (1.0 + u);
+      dp = kap * (u / (1.0 + u) - log1p(u));
+      break;
+    }
+    case AGP_PERIODIC: kap = exp(-0.5 * x); q = kap; break;
+    case AGP_WHITE: kap = (x == 0.0) ? 1.0 : 0.0; break;
+    case AGP_CONSTANT: kap = F.param; dp = 1.0; break;
+    default: kap = d2 + F.param; dp = 1.0; break;  // AGP_LINEAR
+  }
+  if (F.transform == AGP_T_SCALE) {
+    if (F.family == AGP_LINEAR) ds = 2.0 * F.s * x;
+    else if (F.family <= AGP_RQ && F.family != AGP_LINEAR) ds = q * F.s * x;  // d d2 / d s = 2 s x
+  }
+}
+
+// does factor F have per-dimension parameters (ARD v of a distance / Linear factor, or Periodic r)?
+__device__ __forceinline__ bool comp_perdim(const CompFactor& F) {
+  if (F.family == AGP_PERIODIC) return true;
+  return F.transform == AGP_T_ARD && F.family != AGP_WHITE && F.family != AGP_CONSTANT;
+}
+
+// The tiling of composite_gram_kernel over the lower triangle: a 64 x 16*CB tile, 4 x CB elements per thread, fp64
+// accumulators.  Per element: every factor's kappa and derivative pieces, the term products and, by the product rule
+// without dividing by any kappa, v_t prod_{g != f} kappa_g for each factor.  Scalar partials (8 variances, 8 scale and
+// 8 parameter slots, the noise trace and sum alpha) leave the CTA through one atomic each; each factor with
+// per-dimension parameters then takes its own pass over the feature chunks, like grad_reduce_kernel's ARD pass.
+template <int NA> struct CompGradCB { static constexpr int v = NA <= 2 ? 2 : 1; };
+
+template <int NA>
+__device__ __forceinline__ void comp_all_kappa(const CompositeDesc& cd, const double (&x)[NA], double (&kap)[AGP_COMP_MAX]) {
+#pragma unroll
+  for (int f = 0; f < AGP_COMP_MAX; ++f) {
+    double ds, dp, q;
+    kap[f] = 1.0;
+    if (f < cd.nfactors) comp_factor_grad(cd.f[f], comp_pick<double, NA>(x, cd.f[f].acc), kap[f], ds, dp, q);
+  }
+}
+
+// v_t prod_{g in t, g != f} kappa_g
+__device__ __forceinline__ double comp_other(const CompositeDesc& cd, const double (&kap)[AGP_COMP_MAX], int f) {
+  const int t = cd.f[f].term;
+  double o = cd.variance[t];
+#pragma unroll
+  for (int g = 0; g < AGP_COMP_MAX; ++g)
+    if (g < cd.nfactors && g != f && cd.f[g].term == t) o *= kap[g];
+  return o;
+}
+
+template <typename T, int NA, int CB>
+__global__ void __launch_bounds__(256, 1)
+composite_grad_reduce_kernel(const T* __restrict__ Xt, int D, int64_t n, const T* __restrict__ Cinv, int64_t ldc,
+                             const T* __restrict__ alpha, const __grid_constant__ CompositeDesc cd,
+                             double* __restrict__ sums, T* __restrict__ noise_diag) {
+  constexpr int TC = 16 * CB;
+  constexpr int NS = 3 * AGP_COMP_MAX + 2;  // variances, scale slots, parameter slots, noise, alpha
+  const int ti = blockIdx.x, tj = blockIdx.y;
+  const int64_t row0 = (int64_t)ti * RT, col0 = (int64_t)tj * TC;
+  if (col0 > row0 + RT - 1) return;
+  __shared__ T sa[RDC][RT + 1];
+  __shared__ T sb[RDC][TC + 1];
+  __shared__ double sw[NA][RDC];
+  __shared__ double sr[NA][RDC];
+  __shared__ double red[8][NS];
+  __shared__ double sard[2][RDC];
+  const T* __restrict__ Wt = (const T*)cd.w;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+  const int tx = tid & 15, ty = tid >> 4;
+  double acc[NA][4][CB];
+#pragma unroll
+  for (int a = 0; a < NA; ++a)
+#pragma unroll
+    for (int r = 0; r < 4; ++r)
+#pragma unroll
+      for (int c = 0; c < CB; ++c) acc[a][r][c] = 0.0;
+  for (int d0 = 0; d0 < D; d0 += RDC) {
+    const int dc = min(RDC, D - d0);
+    for (int idx = tid; idx < RT * RDC; idx += 256) {
+      const int i = idx / RDC, d = idx - i * RDC;
+      sa[d][i] = (d < dc) ? Xt[(row0 + i) * D + d0 + d] : (T)0;
+    }
+    for (int idx = tid; idx < TC * RDC; idx += 256) {
+      const int i = idx / RDC, d = idx - i * RDC;
+      sb[d][i] = (d < dc) ? Xt[(col0 + i) * D + d0 + d] : (T)0;
+    }
+    for (int idx = tid; idx < NA * RDC; idx += 256) {
+      const int a = idx / RDC, d = idx - a * RDC;
+      sw[a][d] = (d < dc) ? (double)Wt[(int64_t)(2 * a) * D + d0 + d] : 0.0;
+      sr[a][d] = (d < dc) ? (double)Wt[(int64_t)(2 * a + 1) * D + d0 + d] : 0.0;
+    }
+    __syncthreads();
+#pragma unroll 1
+    for (int d = 0; d < dc; ++d) {
+      double xa[4], xb[CB];
+#pragma unroll
+      for (int r = 0; r < 4; ++r) xa[r] = (double)sa[d][tx + 16 * r];
+#pragma unroll
+      for (int c = 0; c < CB; ++c) xb[c] = (double)sb[d][ty + 16 * c];
+#pragma unroll
+      for (int a = 0; a < NA; ++a) {
+        const int kind = cd.acc_kind[a];
+        const double w = sw[a][d];
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int c = 0; c < CB; ++c) {
+            double t;
+            if (kind == COMP_ACC_SQ) t = w * (xa[r] - xb[c]);
+            else if (kind == COMP_ACC_DOT) t = w * w * xa[r] * xb[c];
+            else t = sinpi(w * (xa[r] - xb[c])) * sr[a][d];
+            acc[a][r][c] += (kind == COMP_ACC_DOT) ? t : t * t;
+          }
+      }
+    }
+    __syncthreads();
+  }
+  // element weights w = mult * (alpha_i alpha_j - Cinv_ij), 0 outside the lower triangle / padding
+  double wq[4][CB];
+  double part[NS];
+#pragma unroll
+  for (int q = 0; q < NS; ++q) part[q] = 0.0;
+#pragma unroll 1
+  for (int e = 0; e < 4 * CB; ++e) {
+    const int r = e & 3, c = e >> 2;
+    const int64_t gi = row0 + tx + 16 * r, gj = col0 + ty + 16 * c;
+    double w = 0.0;
+    if (gi < n && gj < n && gj <= gi) {
+      const double ai = (double)alpha[gi], aj = (double)alpha[gj];
+      w = ai * aj - (double)Cinv[gi + gj * ldc];
+      if (gi == gj) {
+        part[NS - 2] += w;
+        part[NS - 1] += ai;
+        if (noise_diag) noise_diag[gi] = (T)(0.5 * w);
+      } else {
+        w *= 2.0;
+      }
+    }
+#pragma unroll
+    for (int q = 0; q < 4 * CB; ++q)
+      if (q == e) wq[q & 3][q >> 2] = w;
+    if (w == 0.0) continue;
+    double x[NA];
+#pragma unroll
+    for (int a = 0; a < NA; ++a) {
+      double y = acc[a][0][0];
+#pragma unroll
+      for (int q = 1; q < 4 * CB; ++q)
+        if (q == e) y = acc[a][q & 3][q >> 2];
+      x[a] = (gi == gj && cd.acc_kind[a] != COMP_ACC_DOT) ? 0.0 : y;
+    }
+    double kap[AGP_COMP_MAX];
+    comp_all_kappa<NA>(cd, x, kap);
+#pragma unroll
+    for (int t = 0; t < AGP_COMP_MAX; ++t) {
+      double pt = 1.0;
+#pragma unroll
+      for (int g = 0; g < AGP_COMP_MAX; ++g)
+        if (g < cd.nfactors && cd.f[g].term == t) pt *= kap[g];
+      part[t] += w * pt;
+    }
+#pragma unroll
+    for (int f = 0; f < AGP_COMP_MAX; ++f) {
+      if (f >= cd.nfactors) continue;
+      double k_, ds, dp, q;  // the derivative pieces are recomputed here rather than kept for every factor (registers)
+      comp_factor_grad(cd.f[f], comp_pick<double, NA>(x, cd.f[f].acc), k_, ds, dp, q);
+      const double o = w * comp_other(cd, kap, f);
+      part[AGP_COMP_MAX + f] += o * ds;
+      part[2 * AGP_COMP_MAX + f] += o * dp;
+    }
+  }
+#pragma unroll
+  for (int q = 0; q < NS; ++q) {
+    const double t = warp_sum_d(part[q]);
+    if (lane == 0) red[wid][q] = t;
+  }
+  __syncthreads();
+  if (tid < NS) {
+    double t = 0.0;
+    for (int w8 = 0; w8 < 8; ++w8) t += red[w8][tid];
+    int slot = -1;
+    if (tid < AGP_COMP_MAX) slot = tid < cd.nterms ? cd.g_var[tid] : -1;
+    else if (tid < 2 * AGP_COMP_MAX) slot = tid - AGP_COMP_MAX < cd.nfactors ? cd.f[tid - AGP_COMP_MAX].g_s : -1;
+    else if (tid < 3 * AGP_COMP_MAX) slot = tid - 2 * AGP_COMP_MAX < cd.nfactors ? cd.f[tid - 2 * AGP_COMP_MAX].g_p : -1;
+    else slot = tid == NS - 2 ? 3 : 4;
+    if (slot >= 0) atomicAdd(&sums[slot], t);
+  }
+  // per-dimension passes, one per factor with ARD v or Periodic r
+#pragma unroll 1
+  for (int f = 0; f < cd.nfactors; ++f) {
+    const CompFactor& F = cd.f[f];
+    if (!comp_perdim(F)) continue;
+    const bool per = F.family == AGP_PERIODIC, lin = F.family == AGP_LINEAR;
+    // coefficient of the element: w v_t prod_{g != f} kappa_g times q (distance ARD) / kappa (Periodic) / 1 (Linear)
+    double coef[4][CB];
+#pragma unroll 1
+    for (int e = 0; e < 4 * CB; ++e) {
+      const int r = e & 3, c = e >> 2;
+      const int64_t gi = row0 + tx + 16 * r;
+      double w = wq[0][0];
+#pragma unroll
+      for (int q = 1; q < 4 * CB; ++q)
+        if (q == e) w = wq[q & 3][q >> 2];
+      double cf = 0.0;
+      if (w != 0.0) {
+        const int64_t gj = col0 + ty + 16 * c;
+        double x[NA];
+#pragma unroll
+        for (int a = 0; a < NA; ++a) {
+          double y = acc[a][0][0];
+#pragma unroll
+          for (int q = 1; q < 4 * CB; ++q)
+            if (q == e) y = acc[a][q & 3][q >> 2];
+          x[a] = (gi == gj && cd.acc_kind[a] != COMP_ACC_DOT) ? 0.0 : y;
+        }
+        double kap[AGP_COMP_MAX];
+        comp_all_kappa<NA>(cd, x, kap);
+        double k_, ds, dp, qf;
+        comp_factor_grad(F, comp_pick<double, NA>(x, F.acc), k_, ds, dp, qf);
+        cf = w * comp_other(cd, kap, f) * (lin ? 1.0 : qf);
+      }
+#pragma unroll
+      for (int q = 0; q < 4 * CB; ++q)
+        if (q == e) coef[q & 3][q >> 2] = cf;
+    }
+    const int a = F.acc;
+    for (int d0 = 0; d0 < D; d0 += RDC) {
+      const int dc = min(RDC, D - d0);
+      __syncthreads();
+      for (int idx = tid; idx < RT * RDC; idx += 256) {
+        const int i = idx / RDC, d = idx - i * RDC;
+        sa[d][i] = (d < dc) ? Xt[(row0 + i) * D + d0 + d] : (T)0;
+      }
+      for (int idx = tid; idx < TC * RDC; idx += 256) {
+        const int i = idx / RDC, d = idx - i * RDC;
+        sb[d][i] = (d < dc) ? Xt[(col0 + i) * D + d0 + d] : (T)0;
+      }
+      if (tid < RDC) {
+        sw[0][tid] = (tid < dc) ? (double)Wt[(int64_t)(2 * a) * D + d0 + tid] : 0.0;
+        sr[0][tid] = (tid < dc) ? (double)Wt[(int64_t)(2 * a + 1) * D + d0 + tid] : 0.0;
+        sard[0][tid] = 0.0;
+        sard[1][tid] = 0.0;
+      }
+      __syncthreads();
+      for (int d = 0; d < dc; ++d) {
+        const double wd = sw[0][d], ri = sr[0][d];
+        double p0 = 0.0, p1 = 0.0;  // p0: d/d transform weight, p1: d/d r (Periodic)
+#pragma unroll
+        for (int r = 0; r < 4; ++r)
+#pragma unroll
+          for (int c = 0; c < CB; ++c) {
+            const double xa = (double)sa[d][tx + 16 * r], xb = (double)sb[d][ty + 16 * c], df = xa - xb;
+            if (per) {
+              double sn, cs;
+              sincospi(wd * df, &sn, &cs);
+              const double sr_ = sn * ri;
+              p1 += coef[r][c] * sr_ * sr_ * ri;
+              p0 -= coef[r][c] * 3.14159265358979323846 * df * sn * cs * ri * ri;
+            } else if (lin) {
+              p0 += coef[r][c] * 2.0 * wd * xa * xb;
+            } else {
+              p0 += coef[r][c] * wd * df * df;
+            }
+          }
+        p0 = warp_sum_d(p0);
+        p1 = warp_sum_d(p1);
+        if (lane == 0) { atomicAdd(&sard[0][d], p0); atomicAdd(&sard[1][d], p1); }
+      }
+      __syncthreads();
+      if (tid < dc) {
+        if (F.transform == AGP_T_ARD) atomicAdd(&sums[F.g_w + d0 + tid], sard[0][tid]);
+        else if (F.transform == AGP_T_SCALE && per) atomicAdd(&sums[F.g_s], sard[0][tid]);
+        if (per) atomicAdd(&sums[F.g_r + d0 + tid], sard[1][tid]);
+      }
+    }
+  }
+}
+
+template <typename T, int NA>
+void launch_composite_grad_na(const T* Xt, int D, int64_t n, int64_t n_pad, const T* Cinv, int64_t ldc, const T* alpha,
+                              const CompositeDesc& cd, double* sums, T* noise_diag, cudaStream_t s) {
+  constexpr int CB = CompGradCB<NA>::v;
+  dim3 grid((unsigned)(n_pad / RT), (unsigned)(n_pad / (16 * CB)));
+  composite_grad_reduce_kernel<T, NA, CB><<<grid, 256, 0, s>>>(Xt, D, n, Cinv, ldc, alpha, cd, sums, noise_diag);
+  agp_count_launch();
+}
+
 }  // namespace
+
+template <typename T>
+void launch_composite_grad_reduce(const T* Xt, int D, int64_t n, int64_t n_pad, const T* Cinv, int64_t ldc, const T* alpha,
+                                  const CompositeDesc& cd, double* sums, T* noise_diag, cudaStream_t s) {
+  if (n_pad <= 0) return;
+  switch (cd.nacc) {
+    case 1: launch_composite_grad_na<T, 1>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+    case 2: launch_composite_grad_na<T, 2>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+    case 3: launch_composite_grad_na<T, 3>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+    case 4: launch_composite_grad_na<T, 4>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+    case 5: launch_composite_grad_na<T, 5>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+    case 6: launch_composite_grad_na<T, 6>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+    case 7: launch_composite_grad_na<T, 7>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+    default: launch_composite_grad_na<T, 8>(Xt, D, n, n_pad, Cinv, ldc, alpha, cd, sums, noise_diag, s); break;
+  }
+}
+template void launch_composite_grad_reduce<float>(const float*, int, int64_t, int64_t, const float*, int64_t, const float*,
+                                                  const CompositeDesc&, double*, float*, cudaStream_t);
+template void launch_composite_grad_reduce<double>(const double*, int, int64_t, int64_t, const double*, int64_t, const double*,
+                                                   const CompositeDesc&, double*, double*, cudaStream_t);
 
 template <typename T>
 void launch_grad_reduce(const T* Xt, int D, int64_t n, int64_t n_pad, const T* Cinv, int64_t ldc, const T* alpha,

@@ -8,6 +8,33 @@
 
 #define AGP_TILE 128
 
+// ---- composite kernels: sum of product terms, K = sum_t v_t prod_{f in t} kappa_f (agp.h agp_kernel_composite) -------
+#define AGP_COMP_MAX 8
+// accumulator kinds: the distances a composite kernel needs, one register block each
+enum { COMP_ACC_SQ = 0,    // sum_d (w_d diff_d)^2           (raw: w = 1, shared by every Scale/None stationary factor)
+       COMP_ACC_DOT = 1,   // sum_d w_d^2 x_d y_d            (raw: w = 1, shared by every Scale/None Linear factor)
+       COMP_ACC_PER = 2 }; // sum_d (sinpi(w_d diff_d) rinv_d)^2   (one per Periodic factor)
+
+struct CompFactor {
+  int family, transform;
+  int acc;      // accumulator slot; -1: Constant (needs none)
+  int term;     // term index
+  double s, s2; // Scale s and s^2 applied to a shared raw accumulator (1 otherwise)
+  double param; // RQ alpha | Linear c | Constant c
+  // gradient slots (indices into grad_out; -1: none): Scale s, param, ARD v base, Periodic r base
+  int g_s, g_p, g_w, g_r;
+};
+
+struct CompositeDesc {  // passed by value (__grid_constant__); per-dimension weights live in a device array
+  int nterms, nfactors, nacc;
+  double variance[AGP_COMP_MAX];
+  int g_var[AGP_COMP_MAX];       // gradient slot of each term's variance
+  CompFactor f[AGP_COMP_MAX];
+  int acc_kind[AGP_COMP_MAX];
+  // device weights (element type T): accumulator a's w at [2a*D, 2a*D + D), its rinv (Periodic) at [(2a+1)*D, ...)
+  const void* w;
+};
+
 struct GramParams {
   int family;        // AGP_SE ...
   double variance;   // sigma_f^2
@@ -23,6 +50,7 @@ struct GramParams {
   const unsigned char* mask_b;
   int64_t noise_off;  // noise_v index offset for the diagonal (block Gram of an extension)
   int64_t diag_off;   // column index offset: column gj of this launch is global column gj + diag_off
+  const CompositeDesc* comp;  // family == AGP_COMPOSITE: host copy of the descriptor (its weights are on the device)
 };
 
 // op(A) is M x K, op(B) is K x N, C is M x N (ldc).  C = beta*C + alpha*op(A)op(B), alpha in {+1,-1}.
@@ -47,7 +75,7 @@ template <typename T> void launch_prep_points(const T* X, int layout, int64_t n,
 template <typename T> void launch_gram(const T* Xa, const T* Xb, int64_t na_pad, int64_t nb_pad, int D,
                                        T* K, int64_t ldk, const GramParams& p, cudaStream_t s);
 template <typename T> void launch_kdiag(const T* Xt, int64_t n, int D, int family, double variance,
-                                        double linear_c, T* out, cudaStream_t s);
+                                        double linear_c, T* out, cudaStream_t s, const CompositeDesc* comp = nullptr);
 // border rows: E[s, j] = Y[j + s*ldy] - mean_j  (j < n, s < S), 0 elsewhere; E is TILE x n_pad at
 // rows [n_pad, n_pad+TILE) of the factor matrix (leading dimension lda).
 template <typename T> void launch_border_init(T* A, int64_t lda, int64_t n, int64_t n_pad, const T* Y,
@@ -121,6 +149,12 @@ template <typename T> void launch_scale_cols(T* B, int64_t ldb, int64_t rows, in
 template <typename T> void launch_grad_reduce(const T* Xt, int D, int64_t n, int64_t n_pad, const T* Cinv, int64_t ldc,
                                               const T* alpha, int family, double linear_c, int want_ard, double* sums,
                                               T* noise_diag, cudaStream_t s);
+// composite kernels (grad.cu): the same reduction for a sum of product terms over untransformed points; sums is indexed
+// by the descriptor's gradient slots (zeroed by the caller) and holds sum_ij w_ij dK_ij/dtheta (times 1/2 by the caller),
+// sums[3] = sum_i W_ii, sums[4] = sum_i alpha_i
+template <typename T> void launch_composite_grad_reduce(const T* Xt, int D, int64_t n, int64_t n_pad, const T* Cinv, int64_t ldc,
+                                                        const T* alpha, const CompositeDesc& cd, double* sums, T* noise_diag,
+                                                        cudaStream_t s);
 template <typename T> void launch_add_diag(T* A, int64_t lda, int64_t n, double v, cudaStream_t s);
 template <typename T> void launch_sumsq(const T* p, int64_t n, double* out, cudaStream_t s);  // out += sum p^2
 template <typename T> void launch_vfe_prep(const T* y, int64_t n, int mean_kind, double mean_c, const T* mean_v,

@@ -32,6 +32,8 @@ typedef struct agp_vfe_post agp_vfe_post; /* device-resident VFE cache (m_e, Lam
 
 enum { AGP_F32 = 0, AGP_F64 = 1 };
 enum { AGP_SE = 0, AGP_MATERN12 = 1, AGP_MATERN32 = 2, AGP_MATERN52 = 3, AGP_LINEAR = 4 };
+/* factor-only families (valid inside an agp_kernel_composite, AGP_ERR_UNSUPPORTED at top level) and the composite tag */
+enum { AGP_RQ = 5, AGP_PERIODIC = 6, AGP_WHITE = 7, AGP_CONSTANT = 8, AGP_COMPOSITE = 9 };
 enum { AGP_T_NONE = 0, AGP_T_SCALE = 1, AGP_T_ARD = 2 };
 enum { AGP_POINT_MAJOR = 0, AGP_FEATURE_MAJOR = 1 };
 enum { AGP_MEM_HOST = 0, AGP_MEM_DEVICE = 1 };
@@ -46,16 +48,47 @@ enum {
   AGP_ERR_INVALID = 6
 };
 
+/* One factor of a composite kernel: a base kernel over its own input transform.  With d2 the squared Euclidean distance
+ * of the transformed inputs x~, y~ (KernelFunctions definitions):
+ *   AGP_SE / AGP_MATERN12 / 32 / 52   as the single-kernel families
+ *   AGP_LINEAR     x~ . y~ + c                                  (param = c)
+ *   AGP_RQ         (1 + d2 / (2 alpha))^(-alpha), alpha > 0     (param = alpha)
+ *   AGP_PERIODIC   exp(-1/2 sum_i (sinpi(x~_i - y~_i) / r_i)^2), r > 0 (r == NULL -> ones)
+ *   AGP_WHITE      1 if x~ == y~, else 0
+ *   AGP_CONSTANT   c                                            (param = c)
+ * with_lengthscale(PeriodicKernel(r), p) is an AGP_PERIODIC factor with ScaleTransform(1/p). */
+typedef struct {
+  int32_t family, transform; /* AGP_SE..AGP_CONSTANT; AGP_T_* of this factor's inputs */
+  double scale;              /* ScaleTransform s */
+  double param;              /* RQ alpha | Linear c | Constant c */
+  const void* ard;           /* ARD v, D values of `dtype`, HOST */
+  const void* r;             /* Periodic r, D values of `dtype`, HOST (NULL -> ones) */
+} agp_kernel_factor;
+
+/* K(x, y) = sum_t variance[t] * prod_{f in term t} kappa_f(T_f x, T_f y): KernelSum / KernelProduct / ScaledKernel trees
+ * flattened into a sum of product terms.  At most 8 terms and 8 factors in all. */
+typedef struct {
+  int32_t nterms;                   /* 1..8 */
+  const int32_t* nfactors;          /* per term, >= 1, total <= 8 */
+  const double* variance;           /* v_t per term */
+  const agp_kernel_factor* factors; /* concatenated term by term */
+} agp_kernel_composite;
+
 /* sigma_f^2 * (kappa o transform): KernelFunctions ScaledKernel / TransformedKernel with
  * ScaleTransform(s) | ARDTransform(v); with_lengthscale(k,l) == scale 1/l.
- * Reference call sites: src/base_gp.jl:70,72,74. */
+ * Reference call sites: src/base_gp.jl:70,72,74.
+ * family == AGP_COMPOSITE: the kernel is `composite` (transform must be AGP_T_NONE and variance 1; scale, linear_c and
+ * ard are ignored).  The single-GPU exact path (agp_gram, agp_fit, agp_rand and the agp_post_* calls on its handle)
+ * accepts it; the VFE entry points and distributed contexts return AGP_ERR_UNSUPPORTED.  Out-of-range counts, a missing
+ * ARD array, alpha <= 0 or r <= 0 give AGP_ERR_INVALID.  `composite` is read only for that family. */
 typedef struct {
-  int32_t family;    /* AGP_SE ... AGP_LINEAR */
+  int32_t family;    /* AGP_SE ... AGP_LINEAR, AGP_COMPOSITE */
   int32_t transform; /* AGP_T_* */
   double variance;   /* sigma_f^2 */
   double scale;      /* ScaleTransform s */
   double linear_c;   /* LinearKernel c */
   const void* ard;   /* ARDTransform v: D values in `dtype`, HOST memory always */
+  const agp_kernel_composite* composite; /* AGP_COMPOSITE only; HOST; copied by the call (handles keep their own copy) */
 } agp_kernel;
 
 /* ZeroMean / ConstMean / CustomMean-evaluated-to-a-vector (src/mean_function.jl:27,40,52-55) */
@@ -152,8 +185,14 @@ int32_t agp_post_rand(agp_post* p, int32_t layout, const void* Xs, int64_t M, co
  * grad_out (double, 5 + D entries): [0] d/d variance, [1] d/d ScaleTransform s, [2] d/d LinearKernel c,
  * [3] d/d sigma^2 (scalar noise; = 1/2 tr W), [4] d/d ConstMean c, [5 + d] d/d ARDTransform v_d.
  * noise_diag_out (N elements of the handle's dtype, or NULL): d/d sigma_i^2 for per-point noise, and -- via
- * d/d m_i = alpha_i -- the caller already holds the gradient w.r.t. a vector mean. */
+ * d/d m_i = alpha_i -- the caller already holds the gradient w.r.t. a vector mean.
+ * Composite handle (AGP_COMPOSITE): grad_out has agp_post_grad_len(p) entries.  [0..2] are 0, [3] and [4] as above, and
+ * from [5] each term in order takes d/d variance[t], then, for each of its factors in order: d/d s (Scale) or d/d v[0..D)
+ * (ARD), then d/d param (RQ alpha, Linear c, Constant c), then d/d r[0..D) (Periodic).  A White factor's entries are 0
+ * (the kernel is piecewise constant in its inputs' transform). */
 int32_t agp_post_logpdf_grad(agp_post* p, double* grad_out, void* noise_diag_out);
+/* number of doubles agp_post_logpdf_grad writes: 5 + D for a single kernel, the layout above for a composite */
+int64_t agp_post_grad_len(const agp_post* p);
 /* V = U' \ B (N x nrhs, column-major): backs Xt_invA_X / diag_Xt_invA_X / Xt_invA_Y /
  * tr_Xt_invA_X on a device factor, src/util/common_covmat_ops.jl:54-60,90,101. */
 int32_t agp_post_solve_lower(agp_post* p, const void* B, int64_t nrhs, void* V_out);

@@ -21,7 +21,10 @@ import Random
 const libagp = get(ENV, "AGP_LIB", "libagp.so")
 
 # ---- POD structs of include/agp.h ------------------------------------------------------------
-struct AgpKernel; family::Int32; transform::Int32; variance::Float64; scale::Float64; linear_c::Float64; ard::Ptr{Cvoid}; end
+struct AgpKernelFactor; family::Int32; transform::Int32; scale::Float64; param::Float64; ard::Ptr{Cvoid}; r::Ptr{Cvoid}; end
+struct AgpKernelComposite; nterms::Int32; nfactors::Ptr{Int32}; variance::Ptr{Float64}; factors::Ptr{AgpKernelFactor}; end
+# `composite` (agp.h agp_kernel_composite) is read only for family AGP_COMPOSITE; single kernels pass C_NULL
+struct AgpKernel; family::Int32; transform::Int32; variance::Float64; scale::Float64; linear_c::Float64; ard::Ptr{Cvoid}; composite::Ptr{AgpKernelComposite}; end
 struct AgpMean;   kind::Int32; c::Float64; v::Ptr{Cvoid}; end
 struct AgpNoise;  kind::Int32; s::Float64; v::Ptr{Cvoid}; end
 const AGP_F32, AGP_F64 = Int32(0), Int32(1)
@@ -57,8 +60,9 @@ const Stationary = Union{SqExponentialKernel,Matern12Kernel,Matern32Kernel,Mater
 family(::SqExponentialKernel) = Int32(0); family(::Matern12Kernel) = Int32(1)
 family(::Matern32Kernel) = Int32(2);      family(::Matern52Kernel) = Int32(3); family(::LinearKernel) = Int32(4)
 
-# Kernels the engine implements: a base kernel wrapped in any nesting of ScaledKernel / TransformedKernel{Scale|ARD}.
-# Everything else (sums, products, periodic, ...) is NOT claimed: the methods below `invoke` the stock reference method.
+# Single kernels the engine implements: a base kernel wrapped in any nesting of ScaledKernel / TransformedKernel{Scale|ARD}.
+# Sums, products and the factor-only families are claimed separately (`composite_supported`, exact path only); everything
+# else is NOT claimed: the methods below `invoke` the stock reference method.
 supported(::Union{Stationary,LinearKernel}) = true
 supported(k::ScaledKernel) = supported(k.kernel)
 supported(k::TransformedKernel{<:Any,<:Union{ScaleTransform,ARDTransform}}) = supported(k.kernel)
@@ -89,11 +93,100 @@ end
 # returns (AgpKernel, keepalive)
 function kernel_spec(k, T)
     fam, var, c, w = flat(k)
-    w === nothing && return (AgpKernel(fam, 0, var, 1.0, c, C_NULL), nothing)
-    w isa Real && return (AgpKernel(fam, 1, var, Float64(w), c, C_NULL), nothing)
+    w === nothing && return (AgpKernel(fam, 0, var, 1.0, c, C_NULL, C_NULL), nothing)
+    w isa Real && return (AgpKernel(fam, 1, var, Float64(w), c, C_NULL, C_NULL), nothing)
     v = convert(Vector{T}, w)
-    return (AgpKernel(fam, 2, var, 1.0, c, pointer(v)), v)
+    return (AgpKernel(fam, 2, var, 1.0, c, pointer(v), C_NULL), v)
 end
+# ---- composite kernels: KernelSum / KernelProduct / ScaledKernel / TransformedKernel trees (agp.h agp_kernel_composite) --
+# The tree is flattened into a sum of product terms exactly as the Python mirror's `_walk` does: a sum concatenates its
+# children's terms, a product distributes over them, a ScaledKernel's sigma^2 multiplies into every term below it and a
+# TransformedKernel's scaling into every factor below it.  Within AGP_COMPOSITE_MAX terms and factors in all, the exact
+# single-GPU methods claim the tree; anything else (and every VFE method) falls through to the stock reference methods.
+const AGP_COMPOSITE = Int32(9)
+const AGP_COMPOSITE_MAX = 8
+const FactorOnly = Union{RationalQuadraticKernel,PeriodicKernel,WhiteKernel,ConstantKernel}
+family(::RationalQuadraticKernel) = Int32(5); family(::PeriodicKernel) = Int32(6)
+family(::WhiteKernel) = Int32(7);             family(::ConstantKernel) = Int32(8)
+
+euclidean(k) = !hasproperty(k, :metric) || nameof(typeof(k.metric)) === :Euclidean
+composite_ok(k::Union{Stationary,LinearKernel,FactorOnly}) = euclidean(k)
+composite_ok(k::ScaledKernel) = composite_ok(k.kernel)
+composite_ok(k::TransformedKernel{<:Any,<:Union{ScaleTransform,ARDTransform}}) = composite_ok(k.kernel)
+composite_ok(k::Union{KernelSum,KernelProduct}) = all(composite_ok, k.kernels)
+composite_ok(::Any) = false
+
+# terms of a tree: [(scalings, factors)], scalings = [(ScaledKernel, path)], factors = [(leaf, path, transforms)],
+# transforms = [(TransformedKernel, path)] innermost first.  A path is the list of child positions from the root (the
+# `kernel` field of a ScaledKernel / TransformedKernel is child 1); the rrule addresses the tangent by it, so a parameter
+# that flattening copies into several terms collects every copy's gradient.
+walk(k::Union{Stationary,LinearKernel,FactorOnly}, p) = Any[(Any[], Any[(k, p, Any[])])]
+walk(k::ScaledKernel, p) = Any[(vcat(Any[(k, p)], s), f) for (s, f) in walk(k.kernel, [p; 1])]
+walk(k::TransformedKernel, p) = Any[(s, Any[(l, lp, vcat(tr, Any[(k, p)])) for (l, lp, tr) in f]) for (s, f) in walk(k.kernel, [p; 1])]
+walk(k::KernelSum, p) = reduce(vcat, [walk(c, [p; i]) for (i, c) in enumerate(k.kernels)])
+function walk(k::KernelProduct, p)
+    terms = Any[(Any[], Any[])]
+    for (i, c) in enumerate(k.kernels)
+        ct = walk(c, [p; i])
+        terms = Any[(vcat(a[1], b[1]), vcat(a[2], b[2])) for a in terms for b in ct]
+    end
+    return terms
+end
+walk(k) = walk(k, Int[])
+
+within_limits(terms) = length(terms) <= AGP_COMPOSITE_MAX && sum(t -> length(t[2]), terms) <= AGP_COMPOSITE_MAX
+composite_supported(k) = !supported(k) && composite_ok(k) && within_limits(walk(k))
+
+# the exact single-GPU methods claim single kernels and composites; the VFE methods keep `supported` (single kernels)
+claimed(f::GP) = (supported(f.kernel) || composite_supported(f.kernel)) && supported(f.mean)
+claimed(::Any) = false
+
+sigma2(s::ScaledKernel) = Float64(only(s.σ²))
+tscale(t::TransformedKernel) = t.transform isa ScaleTransform ? Float64(only(t.transform.s)) : Float64.(t.transform.v)
+prod_except(xs, j, D) = foldl((a, b) -> a .* b, (xs[i] for i in eachindex(xs) if i != j); init=D === nothing ? 1.0 : ones(D))
+
+# (AGP_T_*, s, v) of a factor: its transform chain multiplied out
+function transform_of(tr, D)
+    isempty(tr) && return (Int32(0), 1.0, nothing)
+    ws = [tscale(t) for (t, _) in tr]
+    all(w -> w isa Real, ws) && return (Int32(1), prod(ws), nothing)
+    v = prod_except(ws, 0, D)
+    length(v) == D || throw(DimensionMismatch("ARD weights have length $(length(v)), inputs have D = $D"))
+    return (Int32(2), 1.0, v)
+end
+factor_param(k::RationalQuadraticKernel) = Float64(only(k.α))
+factor_param(k::Union{LinearKernel,ConstantKernel}) = Float64(only(k.c))
+factor_param(::Any) = 0.0
+function periodic_r(k::PeriodicKernel, D)
+    length(k.r) in (1, D) || throw(DimensionMismatch("PeriodicKernel r has length $(length(k.r)), inputs have D = $D"))
+    return length(k.r) == 1 ? fill(Float64(only(k.r)), D) : Float64.(k.r)
+end
+
+# returns (AgpKernel, keepalive) for a composite tree
+function composite_spec(k, T, D)
+    terms = walk(k)
+    keep = Any[]
+    nf = Int32[length(f) for (_, f) in terms]
+    var = Float64[prod(sigma2(s) for (s, _) in sc; init=1.0) for (sc, _) in terms]
+    facs = AgpKernelFactor[]
+    for (_, fs) in terms, (leaf, _, tr) in fs
+        kind, s, v = transform_of(tr, D)
+        ard = C_NULL
+        if v !== nothing
+            va = convert(Vector{T}, v); push!(keep, va); ard = pointer(va)
+        end
+        r = C_NULL
+        if leaf isa PeriodicKernel
+            ra = convert(Vector{T}, periodic_r(leaf, D)); push!(keep, ra); r = pointer(ra)
+        end
+        push!(facs, AgpKernelFactor(family(leaf), kind, s, factor_param(leaf), ard, r))
+    end
+    comp = [AgpKernelComposite(Int32(length(terms)), pointer(nf), pointer(var), pointer(facs))]
+    push!(keep, nf, var, facs, comp)
+    return (AgpKernel(AGP_COMPOSITE, 0, 1.0, 1.0, 0.0, C_NULL, pointer(comp)), keep)
+end
+kernel_spec(k, T, D) = supported(k) ? kernel_spec(k, T) : composite_spec(k, T, D)
+
 mean_spec(::AbstractGPs.ZeroMean, x, T) = (AgpMean(0, 0.0, C_NULL), nothing)
 mean_spec(m::AbstractGPs.ConstMean, x, T) = (AgpMean(1, Float64(m.c), C_NULL), nothing)
 function mean_spec(m::AbstractGPs.CustomMean, x, T)      # arbitrary closure: evaluated host-side
@@ -144,7 +237,7 @@ function fit(fx::DevFiniteGP{T}, Y::AbstractVecOrMat; want_post::Bool=true) wher
     c = ctx()
     X, layout, D = points(fx.x)
     Ym = convert(Matrix{T}, reshape(Y, length(fx), :))
-    ks, k1 = kernel_spec(fx.f.kernel, T); ms, k2 = mean_spec(fx.f.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
+    ks, k1 = kernel_spec(fx.f.kernel, T, D); ms, k2 = mean_spec(fx.f.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
     lp = Vector{T}(undef, size(Ym, 2)); α = Vector{T}(undef, length(fx)); post = Ref{Ptr{Cvoid}}(C_NULL)
     lock(c.lock) do
         GC.@preserve X Ym k1 k2 k3 begin
@@ -165,9 +258,9 @@ end
 # priors the engine does not implement fall through to the reference's own methods (Julia dispatch, not a CPU fallback
 # inside the engine)
 logpdf(fx::DevFiniteGP{T}, Y::AbstractVecOrMat{<:Real}) where {T} =
-    supported(fx.f) ? fit(fx, Y; want_post=false)[1] : invoke(logpdf, Tuple{FiniteGP,typeof(Y)}, fx, Y)
+    claimed(fx.f) ? fit(fx, Y; want_post=false)[1] : invoke(logpdf, Tuple{FiniteGP,typeof(Y)}, fx, Y)
 posterior(fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T} =
-    supported(fx.f) ? fit(fx, y)[2] : invoke(posterior, Tuple{FiniteGP,AbstractVector{<:Real}}, fx, y)
+    claimed(fx.f) ? fit(fx, y)[2] : invoke(posterior, Tuple{FiniteGP,AbstractVector{<:Real}}, fx, y)
 
 # replaces src/exact_gpr_posterior.jl:85-90 (+ src/finite_gp_projection.jl:154-158) with the fused cross-Gram path
 const DevPosterior = PosteriorGP{<:GP,<:NamedTuple{(:α, :C, :x, :δ),<:Tuple{Any,DeviceCholesky,Any,Any}}}
@@ -223,9 +316,9 @@ end
 
 # replaces rand(rng, fx, S) src/finite_gp_projection.jl:233-237: the normals come from the caller's rng
 function Random.rand(rng::Random.AbstractRNG, fx::DevFiniteGP{T}, S::Int) where {T}
-    supported(fx.f) || return invoke(Random.rand, Tuple{Random.AbstractRNG,FiniteGP,Int}, rng, fx, S)
+    claimed(fx.f) || return invoke(Random.rand, Tuple{Random.AbstractRNG,FiniteGP,Int}, rng, fx, S)
     c = ctx(); X, layout, D = points(fx.x); Z = randn(rng, T, length(fx), S); out = similar(Z)
-    ks, k1 = kernel_spec(fx.f.kernel, T); ms, k2 = mean_spec(fx.f.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
+    ks, k1 = kernel_spec(fx.f.kernel, T, D); ms, k2 = mean_spec(fx.f.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
     lock(c.lock) do
         GC.@preserve X k1 k2 k3 check(c, ccall((:agp_rand, libagp), Int32,
             (Ptr{Cvoid}, Int32, Ref{AgpKernel}, Ref{AgpMean}, Ref{AgpNoise}, Int32, Ptr{Cvoid}, Int64, Int32, Ptr{Cvoid}, Int32, Ptr{Cvoid}),
@@ -339,7 +432,86 @@ mean_tangent(m, g) = CRC.NoTangent()
 noise_tangent(Σ::Diagonal{<:Any,<:Fill}, g) = CRC.Tangent{typeof(Σ)}(; diag=CRC.Tangent{typeof(Σ.diag)}(; value=g.noise))
 noise_tangent(Σ::Diagonal, g) = CRC.Tangent{typeof(Σ)}(; diag=collect(g.noise_diag))
 
+# ---- composite kernels: the descriptor gradient (agp.h, agp_post_logpdf_grad) mapped onto the tree by the chain rule ----
+# Slots from g[6] (1-based): per term d/d v_t, then per factor d/d s or d/d v[1:D], d/d param, d/d r[1:D].  v_t is the
+# product of the term's ScaledKernel sigma^2, a factor's s / v the product of its transforms: each node receives the slot's
+# gradient times the product of the OTHER nodes (no division by a parameter), summed over every copy flattening made.
+function composite_grads(k, D, g)
+    acc = Dict{Vector{Int},Any}()
+    add!(p, x) = (acc[p] = haskey(acc, p) ? acc[p] .+ x : x)
+    pos = 6
+    for (sc, fs) in walk(k)
+        σ = [sigma2(s) for (s, _) in sc]
+        for (j, (_, p)) in enumerate(sc)
+            add!(p, g[pos] * prod_except(σ, j, nothing))
+        end
+        pos += 1
+        for (leaf, lp, tr) in fs
+            kind, _, _ = transform_of(tr, D)
+            ws = [tscale(t) for (t, _) in tr]
+            if kind == 1
+                for (j, (_, p)) in enumerate(tr)
+                    add!(p, g[pos] * prod_except(ws, j, nothing))
+                end
+                pos += 1
+            elseif kind == 2
+                gv = g[pos:pos+D-1]
+                for (j, (t, p)) in enumerate(tr)
+                    c = gv .* prod_except(ws, j, D)
+                    add!(p, t.transform isa ScaleTransform ? sum(c) : c)
+                end
+                pos += D
+            end
+            if leaf isa Union{RationalQuadraticKernel,LinearKernel,ConstantKernel}
+                add!(lp, g[pos]); pos += 1
+            end
+            if leaf isa PeriodicKernel
+                gr = g[pos:pos+D-1]
+                add!(lp, length(leaf.r) == 1 ? [sum(gr)] : gr); pos += D
+            end
+        end
+    end
+    return acc
+end
+
+# tangent of the tree from the per-path gradients (scaled by the cotangent d)
+ctangent(k::Union{Stationary,WhiteKernel}, p, acc, d) = CRC.NoTangent()
+ctangent(k::LinearKernel, p, acc, d) = CRC.Tangent{typeof(k)}(; c=[d * get(acc, p, 0.0)])
+ctangent(k::ConstantKernel, p, acc, d) = CRC.Tangent{typeof(k)}(; c=[d * get(acc, p, 0.0)])
+ctangent(k::RationalQuadraticKernel, p, acc, d) = CRC.Tangent{typeof(k)}(; α=[d * get(acc, p, 0.0)])
+ctangent(k::PeriodicKernel, p, acc, d) = CRC.Tangent{typeof(k)}(; r=d .* get(acc, p, zeros(length(k.r))))
+ctangent(k::ScaledKernel, p, acc, d) =
+    CRC.Tangent{typeof(k)}(; kernel=ctangent(k.kernel, [p; 1], acc, d), σ²=[d * get(acc, p, 0.0)])
+ctangent(k::TransformedKernel{<:Any,<:ScaleTransform}, p, acc, d) = CRC.Tangent{typeof(k)}(;
+    kernel=ctangent(k.kernel, [p; 1], acc, d), transform=CRC.Tangent{typeof(k.transform)}(; s=[d * get(acc, p, 0.0)]))
+ctangent(k::TransformedKernel{<:Any,<:ARDTransform}, p, acc, d) = CRC.Tangent{typeof(k)}(;
+    kernel=ctangent(k.kernel, [p; 1], acc, d),
+    transform=CRC.Tangent{typeof(k.transform)}(; v=d .* get(acc, p, zeros(length(k.transform.v)))))
+function ctangent(k::Union{KernelSum,KernelProduct}, p, acc, d)
+    ts = [ctangent(c, [p; i], acc, d) for (i, c) in enumerate(k.kernels)]
+    CRC.Tangent{typeof(k)}(; kernels=k.kernels isa Tuple ? CRC.Tangent{typeof(k.kernels)}(ts...) : ts)
+end
+
+function composite_rrule(fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T}
+    lp, post = fit(fx, y)
+    D = points(fx.x)[3]; N = length(fx); c = ctx()
+    g = Vector{Float64}(undef, ccall((:agp_post_grad_len, libagp), Int64, (Ptr{Cvoid},), post.data.C.h)); nd = Vector{T}(undef, N)
+    lock(c.lock) do
+        GC.@preserve g nd check(c, ccall((:agp_post_logpdf_grad, libagp), Int32, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Cvoid}), post.data.C.h, g, nd))
+    end
+    acc = composite_grads(fx.f.kernel, D, g)
+    function composite_pullback(Δ)
+        d = CRC.unthunk(Δ)
+        gs = (noise=d * g[4], mean_c=d * g[5], noise_diag=d .* nd)
+        f̄ = CRC.Tangent{typeof(fx.f)}(; mean=mean_tangent(fx.f.mean, gs), kernel=ctangent(fx.f.kernel, Int[], acc, d))
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=CRC.NoTangent(), Σy=noise_tangent(fx.Σy, gs))
+        return CRC.NoTangent(), f̄x, -d .* post.data.α
+    end
+    return lp, composite_pullback
+end
+
 function CRC.rrule(::typeof(logpdf), fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T}
+    claimed(fx.f) && !supported(fx.f) && return composite_rrule(fx, y)
     supported(fx.f) || return nothing                                     # no rule: AD differentiates the stock method
     lp, g = logpdf_and_gradient(fx, y)
     _, var, _, w = flat(fx.f.kernel)
