@@ -697,6 +697,8 @@ class FiniteGP:
 
     def __init__(self, f, x, s2=default_s2):
         self.f, self.x = f, _Points(x)
+        # the container the inputs came in, for gradients shaped like it: ColVecs, RowVecs (or a point set) or a vector
+        self.x_kind = "col" if isinstance(x, ColVecs) else ("row" if isinstance(x, (RowVecs, _Points)) else "vec")
         if np.ndim(s2) == 2:
             raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "dense Sigma_y is outside the device hot path (SURVEY s8a)")
         self.s2 = s2
@@ -894,11 +896,15 @@ def fit(fx: FiniteGP, y):
     return _fit(fx, y, True, True)
 
 
-def logpdf_grad(fx: FiniteGP, y):
+def logpdf_grad(fx: FiniteGP, y, inputs=False):
     """EXPERIMENTAL (device path not yet validated): (logpdf, gradient dict) of logpdf(fx, y) w.r.t. the kernel variance,
     ScaleTransform s / ARDTransform v, LinearKernel c, the noise (scalar or per-point) and the mean (constant or vector)
     -- the cotangents Zygote returns through the reference (test/finite_gp_projection.jl:152-178).  One fit, then
-    agp_post_logpdf_grad on its factor."""
+    agp_post_logpdf_grad on its factor.
+
+    inputs=True also returns out["x"], the gradient with respect to the input points, shaped like the container fx was
+    built from (RowVecs: N x D, ColVecs: D x N, a vector: length N) in the handle's dtype; both come from one
+    agp_post_logpdf_grad_x call.  A CustomMean is treated as a constant of x."""
     lp, post = _fit(fx, y, True, True)
     eng = engine()
     f = post.prior
@@ -909,7 +915,18 @@ def logpdf_grad(fx: FiniteGP, y):
     g = np.zeros(int(eng.L.agp_post_grad_len(post.data.C.h)) if composite else 5 + D, dtype=np.float64)
     per_point = np.ndim(fx.s2) != 0
     nd = np.empty(len(fx), dtype=dt) if (per_point or isinstance(f.mean, CustomMean)) else None
-    eng.check(eng.L.agp_post_logpdf_grad(post.data.C.h, g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd)))
+    if inputs:
+        xk = fx.x_kind
+        if xk == "col":
+            layout, xg = cabi.AGP_POINT_MAJOR, np.empty((D, len(fx)), dtype=dt, order="F")
+        elif xk == "vec":
+            layout, xg = cabi.AGP_POINT_MAJOR, np.empty(len(fx), dtype=dt)
+        else:
+            layout, xg = cabi.AGP_FEATURE_MAJOR, np.empty((len(fx), D), dtype=dt, order="F")
+        eng.check(eng.L.agp_post_logpdf_grad_x(post.data.C.h, g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), layout,
+                                               cabi.ptr(xg)))
+    else:
+        eng.check(eng.L.agp_post_logpdf_grad(post.data.C.h, g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd)))
     if composite:
         # composite: out["kernel"][i] is the derivative in kernel_params(k)[i] (the descriptor's gradient mapped back)
         out = {"kernel": _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D).params_grad(g)}
@@ -926,6 +943,8 @@ def logpdf_grad(fx: FiniteGP, y):
         out["mean_c"] = g[4]
     elif isinstance(f.mean, CustomMean):
         out["mean_v"] = post.data.alpha.astype(np.float64)
+    if inputs:
+        out["x"] = xg
     return lp, out
 
 

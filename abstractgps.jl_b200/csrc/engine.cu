@@ -1196,14 +1196,17 @@ int post_cond_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp
 // substitution on the identity, C^-1 = V'V by the lower-only GEMM (both validated kernels), then grad.cu's fused
 // reduction 1/2 sum (alpha alpha' - C^-1) o dC/dtheta.  Extra cost ~ 2 N^3 flop and two N^2 buffers.
 template <typename T>
-int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out) {
+int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, int layout, void* x_grad_out) {
   agp_ctx* ctx = p->ctx;
+  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
   { int rrc = post_replicate<T>(p); if (rrc) return rrc; }
   cudaStream_t s = ctx->stream;
   CK(cudaSetDevice(ctx->device));
   if (p->valid || p->segs.size() > 1) { ctx->err = "gradient of an extended (sequentially conditioned) posterior is unsupported"; return AGP_ERR_UNSUPPORTED; }
   const int64_t n = p->n, n_pad = p->n_pad;
   const int D = p->D;
+  const bool want_theta = grad_out || noise_diag_out;  // the hyper-parameter reduction also yields noise_diag
+  if (!want_theta && !x_grad_out) return AGP_OK;
   Scratch sc(ctx);
   void* tmp = nullptr;
   CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
@@ -1226,21 +1229,56 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out) {
     g.C = Cinv; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = 1;
     launch_gemm<T>(g, s);
   }
+  const int want_ard = (p->k.transform == AGP_T_ARD) ? 1 : 0;
+  if (want_theta) {
+    if (p->comp)
+      launch_composite_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->comp->desc, sums, noise_d, s);
+    else
+      launch_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->k.family, p->k.linear_c, want_ard,
+                            sums, noise_d, s);
+  }
+  if (x_grad_out) {  // sum_j W_ij d1k(x_i, x_j) from the same C^-1 (grad_x.cu)
+    CompositeDesc one{};  // a single kernel is one factor over the transformed points; its chain factor comes last
+    const CompositeDesc* cd = &one;
+    double mult = 1.0;
+    const T* ard = nullptr;
+    if (p->comp) {
+      cd = &p->comp->desc;
+    } else {
+      one.nterms = 1; one.nfactors = 1; one.nacc = 1;
+      one.variance[0] = p->k.variance;
+      one.f[0].family = p->k.family; one.f[0].transform = AGP_T_NONE; one.f[0].acc = 0; one.f[0].term = 0;
+      one.f[0].s = 1.0; one.f[0].s2 = 1.0; one.f[0].param = p->k.linear_c;
+      one.f[0].g_s = one.f[0].g_p = one.f[0].g_w = one.f[0].g_r = -1;
+      one.acc_kind[0] = p->k.family == AGP_LINEAR ? COMP_ACC_DOT : COMP_ACC_SQ;
+      one.w = nullptr;
+      if (p->k.transform == AGP_T_SCALE) mult = p->k.scale;
+      else if (want_ard) ard = (const T*)p->ard;
+    }
+    CK(sc.alloc(&tmp, (size_t)grad_x_part_len(n, D, cd->nacc) * sizeof(double)));
+    double* part = (double*)tmp;
+    CK(sc.alloc(&tmp, (size_t)n * D * sizeof(T)));
+    T* xg = (T*)tmp;
+    launch_grad_x<T>((const T*)p->Xt, D, n, Cinv, n_pad, (const T*)p->alpha, *cd, mult, ard, layout, part, xg, s);
+    int rc = download<T>(ctx, x_grad_out, xg, (size_t)n * D, false); if (rc) return rc;
+  }
+  if (!want_theta) {
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    return AGP_OK;
+  }
   if (p->comp) {  // composite: every kernel slot is 1/2 sum_ij W_ij dK_ij/dtheta, already in its final place
-    launch_composite_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->comp->desc, sums, noise_d, s);
     std::vector<double> h((size_t)nsums);
     CK(cudaMemcpyAsync(h.data(), sums, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
     if (noise_diag_out) { int rc = download<T>(ctx, noise_diag_out, noise_d, (size_t)n, false); if (rc) return rc; }
     CK(cudaStreamSynchronize(s));
     CK(cudaGetLastError());
+    if (!grad_out) return AGP_OK;
     for (int64_t i = 0; i < nsums; ++i) grad_out[i] = 0.5 * h[(size_t)i];
     grad_out[0] = grad_out[1] = grad_out[2] = 0.0;
     grad_out[4] = h[4];
     return AGP_OK;
   }
-  const int want_ard = (p->k.transform == AGP_T_ARD) ? 1 : 0;
-  launch_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->k.family, p->k.linear_c, want_ard,
-                        sums, noise_d, s);
   std::vector<double> h((size_t)5 + D);
   std::vector<T> ard_h((size_t)(D > 0 ? D : 1));
   CK(cudaMemcpyAsync(h.data(), sums, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
@@ -1248,6 +1286,7 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out) {
   if (noise_diag_out) { int rc = download<T>(ctx, noise_diag_out, noise_d, (size_t)n, false); if (rc) return rc; }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
+  if (!grad_out) return AGP_OK;
   const bool linear = p->k.family == AGP_LINEAR;
   const double var = p->k.variance, sc_ = p->k.scale;
   grad_out[0] = 0.5 * h[0];
@@ -2475,8 +2514,13 @@ int32_t agp_post_rand(agp_post* p, int32_t layout, const void* Xs, int64_t M, co
 
 int32_t agp_post_logpdf_grad(agp_post* p, double* grad_out, void* noise_diag_out) {
   if (!p || !grad_out) return AGP_ERR_INVALID;
-  return DISPATCH(p->dtype, post_logpdf_grad_impl<float>(p, grad_out, noise_diag_out),
-                  post_logpdf_grad_impl<double>(p, grad_out, noise_diag_out));
+  return agp_post_logpdf_grad_x(p, grad_out, noise_diag_out, AGP_POINT_MAJOR, nullptr);
+}
+
+int32_t agp_post_logpdf_grad_x(agp_post* p, double* grad_out, void* noise_diag_out, int32_t layout, void* x_grad_out) {
+  if (!p) return AGP_ERR_INVALID;
+  return DISPATCH(p->dtype, post_logpdf_grad_impl<float>(p, grad_out, noise_diag_out, layout, x_grad_out),
+                  post_logpdf_grad_impl<double>(p, grad_out, noise_diag_out, layout, x_grad_out));
 }
 
 int32_t agp_post_solve_lower(agp_post* p, const void* B, int64_t nrhs, void* V_out) {

@@ -155,6 +155,13 @@ template <typename T> void launch_grad_reduce(const T* Xt, int D, int64_t n, int
 template <typename T> void launch_composite_grad_reduce(const T* Xt, int D, int64_t n, int64_t n_pad, const T* Cinv, int64_t ldc,
                                                         const T* alpha, const CompositeDesc& cd, double* sums, T* noise_diag,
                                                         cudaStream_t s);
+// input gradient (grad_x.cu): out (n x D values in `layout`, agp.h) = mult * chain_d * sum_j W_ij d1k(x_i, x_j)_d over the
+// descriptor cd on the points X (n x D, point-major); chain_d = ard[d], or 1 when ard is null.  part: workspace of
+// grad_x_part_len(n, D, cd.nacc) doubles (zeroed inside)
+int64_t grad_x_part_len(int64_t n, int D, int nacc);
+template <typename T> void launch_grad_x(const T* X, int D, int64_t n, const T* Cinv, int64_t ldc, const T* alpha,
+                                         const CompositeDesc& cd, double mult, const T* ard, int layout, double* part,
+                                         T* out, cudaStream_t s);
 template <typename T> void launch_add_diag(T* A, int64_t lda, int64_t n, double v, cudaStream_t s);
 template <typename T> void launch_sumsq(const T* p, int64_t n, double* out, cudaStream_t s);  // out += sum p^2
 template <typename T> void launch_vfe_prep(const T* y, int64_t n, int mean_kind, double mean_c, const T* mean_v,

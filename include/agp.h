@@ -191,6 +191,27 @@ int32_t agp_post_rand(agp_post* p, int32_t layout, const void* Xs, int64_t M, co
  * (ARD), then d/d param (RQ alpha, Linear c, Constant c), then d/d r[0..D) (Periodic).  A White factor's entries are 0
  * (the kernel is piecewise constant in its inputs' transform). */
 int32_t agp_post_logpdf_grad(agp_post* p, double* grad_out, void* noise_diag_out);
+/* The same gradient and, in the same call, the gradient of logpdf(fx, y) with respect to the input points -- what
+ * reverse-mode AD returns for `x` through the reference's logpdf (test/finite_gp_projection.jl:162-173), and what trains
+ * a feature network under the GP (examples/2-deep-kernel-learning).  With W = alpha alpha' - C^-1, for point i and
+ * input dimension d:
+ *   x_grad[i, d] = sum_j W_ij d1k(x_i, x_j)_d      (j over all points, j == i included)
+ * d1 the derivative in the FIRST argument, taken with respect to the untransformed input (the Scale / ARD chain factor
+ * is included).  Per factor, leaving out the variances (with t the Scale s, the ARD v or 1, x~ = t x):
+ *   SE / Matern / RQ   2 kappa'(d2) t^2 (x_i - x_j)          Linear   t^2 x_j   (so the diagonal term t^2 x_i counts)
+ *   Periodic           kappa (-pi t_d / (2 r_d^2)) sinpi(2 t_d (x_i - x_j)_d)   White / Constant   0
+ * and the product rule over a composite's terms.  Coincident points (x~_i == x~_j, i == j included) contribute exactly 0
+ * for every stationary factor: the limit for SE, Matern 3/2 and 5/2, RQ and Periodic, and the zero subgradient of
+ * Matern 1/2, which is not differentiable there.  Finite inputs never give NaN.  Summed in fp64 whatever the dtype, in a
+ * fixed order: two calls on the same handle give the same bits.
+ * grad_out and noise_diag_out are as agp_post_logpdf_grad's; either may be NULL (that part is then not reduced).
+ * x_grad_out: N x D values of the handle's dtype in `layout` -- AGP_POINT_MAJOR: D x N column-major, AGP_FEATURE_MAJOR:
+ * N x D column-major; a DEVICE pointer under AGP_MEM_DEVICE; NULL: not computed.  C^-1 (the ~N^3 part) is formed once
+ * for everything requested.  Like agp_post_logpdf_grad this is the gradient for the one column of Y whose alpha the
+ * handle holds, and only for a handle straight from agp_fit: an extended handle gives AGP_ERR_UNSUPPORTED.  A layout
+ * other than the two gives AGP_ERR_INVALID.  agp_post_logpdf_grad(p, g, nd) is agp_post_logpdf_grad_x(p, g, nd,
+ * AGP_POINT_MAJOR, NULL). */
+int32_t agp_post_logpdf_grad_x(agp_post* p, double* grad_out, void* noise_diag_out, int32_t layout, void* x_grad_out);
 /* number of doubles agp_post_logpdf_grad writes: 5 + D for a single kernel, the layout above for a composite */
 int64_t agp_post_grad_len(const agp_post* p);
 /* V = U' \ B (N x nrhs, column-major): backs Xt_invA_X / diag_Xt_invA_X / Xt_invA_Y /

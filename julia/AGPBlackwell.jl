@@ -396,8 +396,10 @@ AbstractGPs.var(fx::FiniteGP{<:DeviceApproxPosterior}) = mean_and_var(fx)[2]
 # agp_post_logpdf_grad returns, from the factor of ONE fit, d logpdf / d (total sigma_f^2, total ScaleTransform factor,
 # LinearKernel c, scalar noise, constant mean, total ARD weights) and the per-point noise gradient.  `logpdf_and_gradient`
 # exposes them flat; the `rrule` maps them back onto the nested kernel structs (chain rule through the products the shim
-# forms in `flat`: sigma_f^2 = prod of the ScaledKernel factors, w = prod of the transform scalings).  Inputs x are treated
-# as constants (NoTangent); a CustomMean closure is not differentiated.
+# forms in `flat`: sigma_f^2 = prod of the ScaledKernel factors, w = prod of the transform scalings).  The rrules take the
+# same gradients and, from the same C^-1, the gradient with respect to the inputs x through one agp_post_logpdf_grad_x call
+# (`logpdf_gradients`), so a network that computes x (examples/2-deep-kernel-learning) trains through the GP term.  A
+# CustomMean closure is not differentiated (with respect to its parameters or to x).
 import ChainRulesCore
 const CRC = ChainRulesCore
 
@@ -411,6 +413,25 @@ function logpdf_and_gradient(fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) wher
     end
     return lp, (variance=g[1], scale=g[2], linear_c=g[3], noise=g[4], mean_c=g[5], ard=g[6:end], noise_diag=nd, y=-post.data.α)
 end
+
+# the rrules' single call: (lp, post, g, noise_diag, x gradient shaped like fx.x's storage) from one fit and ONE
+# agp_post_logpdf_grad_x (C^-1 is formed once for the hyper-parameters and the inputs); glen = length of g
+function logpdf_gradients(fx::DevFiniteGP{T}, y::AbstractVector{<:Real}, glen) where {T}
+    lp, post = fit(fx, y)
+    X, layout, D = points(fx.x); N = length(fx)
+    g = Vector{Float64}(undef, glen(post, D)); nd = Vector{T}(undef, N); xg = similar(X, T)
+    c = ctx()
+    lock(c.lock) do
+        GC.@preserve g nd xg check(c, ccall((:agp_post_logpdf_grad_x, libagp), Int32,
+            (Ptr{Cvoid}, Ptr{Float64}, Ptr{Cvoid}, Int32, Ptr{Cvoid}), post.data.C.h, g, nd, layout, xg))
+    end
+    return lp, post, g, nd, xg
+end
+
+# tangent of the inputs: the container's own field for ColVecs / RowVecs, a plain vector otherwise
+x_tangent(x::ColVecs, xg) = CRC.Tangent{typeof(x)}(; X=xg)
+x_tangent(x::RowVecs, xg) = CRC.Tangent{typeof(x)}(; X=xg)
+x_tangent(x::AbstractVector{<:Real}, xg) = xg
 
 # tangent of a (nested) kernel: `tot` carries the flattened totals the gradients refer to
 kernel_tangent(k::Stationary, g, var, w) = CRC.NoTangent()
@@ -493,18 +514,14 @@ function ctangent(k::Union{KernelSum,KernelProduct}, p, acc, d)
 end
 
 function composite_rrule(fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T}
-    lp, post = fit(fx, y)
-    D = points(fx.x)[3]; N = length(fx); c = ctx()
-    g = Vector{Float64}(undef, ccall((:agp_post_grad_len, libagp), Int64, (Ptr{Cvoid},), post.data.C.h)); nd = Vector{T}(undef, N)
-    lock(c.lock) do
-        GC.@preserve g nd check(c, ccall((:agp_post_logpdf_grad, libagp), Int32, (Ptr{Cvoid}, Ptr{Float64}, Ptr{Cvoid}), post.data.C.h, g, nd))
-    end
+    D = points(fx.x)[3]
+    lp, post, g, nd, xg = logpdf_gradients(fx, y, (post, D) -> ccall((:agp_post_grad_len, libagp), Int64, (Ptr{Cvoid},), post.data.C.h))
     acc = composite_grads(fx.f.kernel, D, g)
     function composite_pullback(Δ)
         d = CRC.unthunk(Δ)
         gs = (noise=d * g[4], mean_c=d * g[5], noise_diag=d .* nd)
         f̄ = CRC.Tangent{typeof(fx.f)}(; mean=mean_tangent(fx.f.mean, gs), kernel=ctangent(fx.f.kernel, Int[], acc, d))
-        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=CRC.NoTangent(), Σy=noise_tangent(fx.Σy, gs))
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, d .* xg), Σy=noise_tangent(fx.Σy, gs))
         return CRC.NoTangent(), f̄x, -d .* post.data.α
     end
     return lp, composite_pullback
@@ -513,14 +530,15 @@ end
 function CRC.rrule(::typeof(logpdf), fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T}
     claimed(fx.f) && !supported(fx.f) && return composite_rrule(fx, y)
     supported(fx.f) || return nothing                                     # no rule: AD differentiates the stock method
-    lp, g = logpdf_and_gradient(fx, y)
+    lp, post, gv, nd, xg = logpdf_gradients(fx, y, (post, D) -> 5 + D)
+    g = (variance=gv[1], scale=gv[2], linear_c=gv[3], noise=gv[4], mean_c=gv[5], ard=gv[6:end], noise_diag=nd, y=-post.data.α)
     _, var, _, w = flat(fx.f.kernel)
     w === nothing && (w = 1.0)
     function logpdf_pullback(Δ)
         d = CRC.unthunk(Δ)
         gs = map(v -> v isa Number ? d * v : d .* v, g)
         f̄ = CRC.Tangent{typeof(fx.f)}(; mean=mean_tangent(fx.f.mean, gs), kernel=kernel_tangent(fx.f.kernel, gs, var, w))
-        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=CRC.NoTangent(), Σy=noise_tangent(fx.Σy, gs))
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, d .* xg), Σy=noise_tangent(fx.Σy, gs))
         return CRC.NoTangent(), f̄x, gs.y
     end
     return lp, logpdf_pullback
