@@ -1265,6 +1265,54 @@ def elbo(vfe: VFE, fx: FiniteGP, y):
     return approx_log_evidence(vfe, fx, y)
 
 
+def approx_log_evidence_grad(vfe: VFE, fx: FiniteGP, y):
+    """(value, gradient dict) of approx_log_evidence(vfe, fx, y) -- the elbo for VFE, the DTC objective for DTC -- through
+    one agp_vfe_elbo_grad call: what Zygote returns through the reference when a sparse GP is trained.  The dict has the
+    keys of logpdf_grad ("variance", "scale" | "ard", "linear_c", "noise" scalar or per-point, "mean_c" | "mean_v") and
+    "z", the gradient with respect to the inducing points, shaped like the container vfe.fz was built from (RowVecs: M x D,
+    ColVecs: D x M, a vector: length M) in the objective's dtype.  A CustomMean is treated as a constant of x."""
+    eng = engine()
+    f, dt, pts, z, y, ks, ms, ns, js, keep = _vfe_args(vfe, fx, y)
+    D = pts.D
+    k = f.kernel
+    if isinstance(k, _CompositeKernel) or k.family > LINEAR:
+        raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "composite kernels are supported on the exact path only (not VFE)")
+    value = np.empty(1, dtype=dt)
+    g = np.zeros(5 + D, dtype=np.float64)
+    per_point = np.ndim(fx.s2) != 0
+    nd = np.empty(pts.n, dtype=dt) if per_point else None
+    md = np.empty(pts.n, dtype=dt) if isinstance(f.mean, CustomMean) else None
+    # the points go in point-major, so z comes back point-major: D x M column-major, i.e. M x D row-major
+    zg = {"col": lambda: np.empty((D, z.n), dtype=dt, order="F"), "vec": lambda: np.empty(z.n, dtype=dt),
+          "row": lambda: np.empty((z.n, D), dtype=dt)}[vfe.fz.x_kind]()
+    objective = 1 if isinstance(vfe, DTC) else 0
+    eng.check(eng.L.agp_vfe_elbo_grad(eng.h, cabi.dtype_code(dt), C.byref(ks), C.byref(ms), C.byref(ns),
+                                      cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), pts.n, pts.D, cabi.ptr(z.a), z.n, C.byref(js),
+                                      cabi.ptr(y), objective, cabi.ptr(value), g.ctypes.data_as(C.POINTER(C.c_double)),
+                                      cabi.ptr(nd), cabi.ptr(md), cabi.ptr(zg)))
+    out = {"variance": g[0]}
+    if isinstance(k.transform, ScaleTransform):
+        out["scale"] = g[1]
+    elif isinstance(k.transform, ARDTransform):
+        out["ard"] = g[5:5 + D].copy()
+    if k.family == LINEAR:
+        out["linear_c"] = g[2]
+    out["noise"] = nd.astype(np.float64) if per_point else g[3]
+    if isinstance(f.mean, ConstMean):
+        out["mean_c"] = g[4]
+    elif isinstance(f.mean, CustomMean):
+        out["mean_v"] = md.astype(np.float64)
+    out["z"] = zg
+    return value[0], out
+
+
+def elbo_grad(vfe: VFE, fx: FiniteGP, y):
+    """(elbo, gradient dict) of elbo(vfe::VFE, fx, y); VFE only, as elbo.  See approx_log_evidence_grad."""
+    if isinstance(vfe, DTC):
+        raise TypeError("elbo is defined for VFE; use approx_log_evidence for DTC")
+    return approx_log_evidence_grad(vfe, fx, y)
+
+
 def _vfe_posterior(vfe: VFE, fx: FiniteGP, y):
     eng = engine()
     f, dt, pts, z, y, ks, ms, ns, js, keep = _vfe_args(vfe, fx, y)

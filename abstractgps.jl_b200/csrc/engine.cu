@@ -12,6 +12,7 @@
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
+#include <functional>
 #include <string>
 #include <type_traits>
 #include <utility>
@@ -1195,6 +1196,20 @@ int post_cond_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp
 // factor agp_fit left in the handle (SURVEY s8f rank 1).  V = L^-1 by the blocked forward
 // substitution on the identity, C^-1 = V'V by the lower-only GEMM (both validated kernels), then grad.cu's fused
 // reduction 1/2 sum (alpha alpha' - C^-1) o dC/dtheta.  Extra cost ~ 2 N^3 flop and two N^2 buffers.
+// a single kernel as a one-factor descriptor over its transformed points (grad_x.cu); its Scale / ARD chain factor is
+// applied by the caller
+static CompositeDesc single_kernel_desc(int family, double variance, double linear_c) {
+  CompositeDesc one{};
+  one.nterms = 1; one.nfactors = 1; one.nacc = 1;
+  one.variance[0] = variance;
+  one.f[0].family = family; one.f[0].transform = AGP_T_NONE; one.f[0].acc = 0; one.f[0].term = 0;
+  one.f[0].s = 1.0; one.f[0].s2 = 1.0; one.f[0].param = linear_c;
+  one.f[0].g_s = one.f[0].g_p = one.f[0].g_w = one.f[0].g_r = -1;
+  one.acc_kind[0] = family == AGP_LINEAR ? COMP_ACC_DOT : COMP_ACC_SQ;
+  one.w = nullptr;
+  return one;
+}
+
 template <typename T>
 int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, int layout, void* x_grad_out) {
   agp_ctx* ctx = p->ctx;
@@ -1238,20 +1253,13 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, i
                             sums, noise_d, s);
   }
   if (x_grad_out) {  // sum_j W_ij d1k(x_i, x_j) from the same C^-1 (grad_x.cu)
-    CompositeDesc one{};  // a single kernel is one factor over the transformed points; its chain factor comes last
+    const CompositeDesc one = single_kernel_desc(p->k.family, p->k.variance, p->k.linear_c);
     const CompositeDesc* cd = &one;
     double mult = 1.0;
     const T* ard = nullptr;
     if (p->comp) {
       cd = &p->comp->desc;
     } else {
-      one.nterms = 1; one.nfactors = 1; one.nacc = 1;
-      one.variance[0] = p->k.variance;
-      one.f[0].family = p->k.family; one.f[0].transform = AGP_T_NONE; one.f[0].acc = 0; one.f[0].term = 0;
-      one.f[0].s = 1.0; one.f[0].s2 = 1.0; one.f[0].param = p->k.linear_c;
-      one.f[0].g_s = one.f[0].g_p = one.f[0].g_w = one.f[0].g_r = -1;
-      one.acc_kind[0] = p->k.family == AGP_LINEAR ? COMP_ACC_DOT : COMP_ACC_SQ;
-      one.w = nullptr;
       if (p->k.transform == AGP_T_SCALE) mult = p->k.scale;
       else if (want_ard) ard = (const T*)p->ard;
     }
@@ -1587,10 +1595,23 @@ int gram_impl(agp_ctx* ctx, const agp_kernel* k, int layout, const void* X, int6
 // :58-75 (posterior), but STREAMS the data dimension: K_zx is generated chunk by chunk, scaled by
 // Sigma_y^-1/2, solved against chol(K_zz) and folded into D = A A' (M x M), b = A delta and ||A||_F^2,
 // so the M x N matrix A (32.8 GB at config C5) never exists.
+//
+// What the gradient (vfe_grad_impl) needs from the pass: the factors, m_e, D = Lam - I, the prepared points and the
+// per-point vectors.  `after` runs while they are alive; without it the pass launches exactly what the objectives need.
+template <typename T>
+struct VfePass {
+  int64_t N, M, m_pad, lda, cap;
+  int D;
+  const T *Lz, *Dz, *Lm, *Dl, *me, *Dcopy, *Zt, *Xt, *kd, *delta, *isn, *noise_v, *ard;
+  T* B;  // pass 1's chunk buffer (m_pad x cap), free for reuse
+  double noise_s, elbo, dtc;
+};
+template <typename T> using VfeAfter = std::function<int(const VfePass<T>&)>;
+
 template <typename T>
 int vfe_core(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout,
              const void* X, int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y,
-             void* elbo_out, void* dtc_out, agp_vfe_post** post_out) {
+             void* elbo_out, void* dtc_out, agp_vfe_post** post_out, const VfeAfter<T>* after = nullptr) {
   if (k && k->family == AGP_COMPOSITE) {
     ctx->err = "composite kernels are supported on the exact path only (not VFE)";
     return AGP_ERR_UNSUPPORTED;
@@ -1719,11 +1740,17 @@ int vfe_core(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
   CK(cudaEventRecord(ctx->ev[2], s));
 
   // (3) Lambda = chol(D + I), with b riding in the border row
+  T* Dcopy = nullptr;
+  if (after) {
+    CK(sc.alloc(&tmp, (size_t)lda * m_pad * sizeof(T)));
+    Dcopy = (T*)tmp;
+    CK(cudaMemcpyAsync(Dcopy, Lm, (size_t)lda * m_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+  }
   launch_add_diag<T>(Lm, lda, m_pad, 1.0, s);
   launch_border_init<T>(Lm, lda, m_pad, m_pad, bvec, m_pad, 1, 0, 0.0, (const T*)nullptr, s);
   cholesky_inplace<T>(ctx, Lm, lda, m_pad, lda, Dl, ld_l, dinfo);
   launch_extract_v<T>(Lm, lda, m_pad, 1, rwork, sq, s);
-  if (keep) {
+  if (keep || after) {
     CK(sc.alloc(&tmp, (size_t)(nblk + 1) * sizeof(int)));
     int* dflags = (int*)tmp;
     launch_bwd_solve<T>(Lm, lda, Dl, nblk, rwork, dflags, s);       // m_e = Lambda^-1 b
@@ -1756,8 +1783,231 @@ int vfe_core(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
   T e = (T)elbo, dd = (T)dtc;
   if (elbo_out) memcpy(elbo_out, &e, sizeof(T));
   if (dtc_out) memcpy(dtc_out, &dd, sizeof(T));
+  if (after) {
+    const VfePass<T> st{N, M, m_pad, lda, cap, D, Lz, Dz, Lm, Dl, bvec, Dcopy, Zt, Xt, kd, delta, isn, noise_d, ard_d,
+                        B, noise->s, elbo, dtc};
+    rc = (*after)(st);
+    if (rc) return fail(rc);
+  }
   vguard.p = nullptr;
   if (keep) *post_out = vp;
+  return AGP_OK;
+}
+
+// ---- gradient of the VFE objectives (agp_vfe_elbo_grad; the formulas are in agp.h and vfe_grad.cu) ----------------
+// Pass 1 is vfe_core's.  Then, once: V_z = L_z^-1 and V_m = L_m^-1 by the forward substitution on the identity,
+// Lam^-1 = V_m' V_m, H and E, R = V_z' H V_z, P = V_z' E V_z = -2 Kbar_zz and r = V_z' m_e (O(M^3), tile GEMMs).  The K_zz
+// part goes through the exact path's reductions with alpha = 0 and C^-1 = P: grad_reduce_kernel gives
+// 1/2 sum (-P) o dK_zz = sum Kbar_zz o dK_zz, grad_x_kernel gives sum_m' (-P) d1k = 2 sum Kbar_zz d1k.  Pass 2 streams the
+// data in pass 1's chunks: K_zx,c by the Gram kernel, G = R K_zx,c by the tile GEMM, then vfe_cross_grad_kernel and
+// vfe_point_grad_kernel.
+template <typename T>
+int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout,
+                  const void* X, int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y,
+                  int objective, void* value_out, double* grad_out, void* noise_diag_out, void* mean_diag_out,
+                  void* z_grad_out) {
+  if (objective != 0 && objective != 1) { ctx->err = "objective must be 0 (elbo) or 1 (DTC)"; return AGP_ERR_INVALID; }
+  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
+  if (k && k->family == AGP_COMPOSITE) { ctx->err = "composite kernels are supported on the exact path only (not VFE)"; return AGP_ERR_UNSUPPORTED; }
+  if (ctx->nccl) { ctx->err = "the VFE gradient runs on a single-GPU context"; return AGP_ERR_UNSUPPORTED; }
+  const double c = objective == 0 ? 1.0 : 0.0;
+  const VfeAfter<T> grad = [&](const VfePass<T>& p) -> int {
+    cudaStream_t s = ctx->stream;
+    const int64_t mp = p.m_pad, mm = mp * mp;
+    const bool linear = k->family == AGP_LINEAR;
+    const int want_ard = k->transform == AGP_T_ARD ? 1 : 0;
+    Scratch sc(ctx);
+    void* tmp = nullptr;
+    CK(sc.alloc(&tmp, (size_t)(mm * 6 + mp * 2) * sizeof(T)));
+    T* Vz = (T*)tmp; T* W1 = Vz + mm; T* Li = W1 + mm; T* H = Li + mm; T* E = H + mm; T* R = E + mm;
+    T* rv = R + mm; T* az = rv + mp;
+    T* P = H;  // V_z' E V_z takes H's place once R is formed
+    auto gemm = [&](const T* A, int ak, const T* B, int bk, T* C) {
+      GemmArgs g{};
+      g.A = A; g.lda = mp; g.a_kmajor = ak;
+      g.B = B; g.ldb = mp; g.b_kmajor = bk;
+      g.C = C; g.ldc = mp; g.M = mp; g.N = mp; g.K = mp;
+      launch_gemm<T>(g, s);
+    };
+    CK(cudaMemsetAsync(Vz, 0, (size_t)mm * 2 * sizeof(T), s));
+    CK(cudaMemsetAsync(az, 0, (size_t)mp * sizeof(T), s));
+    launch_add_diag<T>(Vz, mp, mp, 1.0, s);
+    launch_add_diag<T>(W1, mp, mp, 1.0, s);
+    forward_subst_multi<T>(ctx, p.Lz, p.lda, p.Dz, mp, Vz, mp, mp);  // V_z
+    forward_subst_multi<T>(ctx, p.Lm, p.lda, p.Dl, mp, W1, mp, mp);  // V_m
+    gemm(W1, 1, W1, 1, Li);                                           // Lam^-1 = V_m' V_m
+    launch_vfe_hz<T>(Li, p.Dcopy, p.lda, p.me, M, mp, c, H, E, s);
+    gemm(H, 0, Vz, 1, W1);
+    gemm(Vz, 1, W1, 1, R);                                            // R = V_z' H V_z
+    gemm(E, 0, Vz, 1, W1);
+    gemm(Vz, 1, W1, 1, P);                                            // P = V_z' E V_z
+    launch_gemv_t<T>(Vz, mp, mp, mp, p.me, 0, 0.0, (const T*)nullptr, rv, s);  // r = V_z' m_e
+
+    const int nsums = 5 + D;
+    CK(sc.alloc(&tmp, (size_t)(nsums + 2) * sizeof(double)));
+    double* sums = (double*)tmp;
+    double* nm = sums + nsums;
+    CK(cudaMemsetAsync(sums, 0, (size_t)(nsums + 2) * sizeof(double), s));
+    launch_grad_reduce<T>(p.Zt, D, M, mp, P, mp, az, k->family, k->linear_c, want_ard, sums, (T*)nullptr, s);
+    const double mult = k->transform == AGP_T_SCALE ? k->scale : 1.0;
+    const T* ard = want_ard ? p.ard : nullptr;
+    T *zz = nullptr, *zout = nullptr;
+    if (z_grad_out) {  // K_zz part of the inducing-point gradient, in the caller's layout
+      const CompositeDesc one = single_kernel_desc(k->family, k->variance, k->linear_c);
+      CK(sc.alloc(&tmp, (size_t)grad_x_part_len(M, D, 1) * sizeof(double)));
+      double* part = (double*)tmp;
+      CK(sc.alloc(&tmp, (size_t)M * D * 2 * sizeof(T)));
+      zz = (T*)tmp; zout = zz + M * D;
+      launch_grad_x<T>(p.Zt, D, M, P, mp, az, one, mult, ard, layout, part, zz, s);
+    }
+
+    // pass 2
+    const int64_t cap = p.cap;
+    int nrb = 0, nsplit = 0;
+    vfe_cross_shape(mp, cap, &nrb, &nsplit);
+    CK(sc.alloc(&tmp, (size_t)mp * cap * sizeof(T)));
+    T* Bk = p.B; T* G = (T*)tmp;
+    // G on the int8-slice general product wherever pass 1 runs its long-K product on the tensor cores (the same rule):
+    // R is sliced once into rows [0, m_pad) of the workspace, each chunk of K_zx behind it
+    constexpr int is_f32 = std::is_same<T, double>::value ? 0 : 1;
+    bool g_tc = resolve_tensor_mode<T>(ctx, (int64_t)1 << 20) == 1 && mp >= 1024 && mp <= 32768 &&
+                ensure_oz2(ctx, mp + cap, (int)mp, slices_of<T>(ctx), s) && ctx->oz2.bulk == 2;
+    if (g_tc) ozaki_prepare_ex(ctx->oz2, R, is_f32, 0, mp, mp, 0, s);
+    CK(sc.alloc(&tmp, (size_t)(2 * nrb * cap + (int64_t)nsplit * D * mp) * sizeof(double)));
+    double* qpart = (double*)tmp; double* upart = qpart + nrb * cap; double* zpart = upart + nrb * cap;
+    CK(cudaMemsetAsync(zpart, 0, (size_t)nsplit * D * mp * sizeof(double), s));
+    T *nd = nullptr, *md = nullptr;
+    if (noise_diag_out) { CK(sc.alloc(&tmp, (size_t)N * sizeof(T))); nd = (T*)tmp; }
+    if (mean_diag_out) { CK(sc.alloc(&tmp, (size_t)N * sizeof(T))); md = (T*)tmp; }
+    for (int64_t c0 = 0; c0 < N; c0 += cap) {
+      const int64_t nc = (N - c0 < cap) ? (N - c0) : cap;
+      const int64_t nc_pad = round_up(nc, TILE);
+      GramParams gx{};
+      fill_gram_params<T>(gx, k, 0, 0, M, nc, nullptr, nullptr);
+      launch_gram<T>(p.Zt, p.Xt + c0 * D, mp, nc_pad, D, Bk, mp, gx, s);
+      bool done = false;
+      if (g_tc) {  // G = R K_zx,c
+        CK(cudaMemsetAsync(G, 0, (size_t)mp * nc_pad * sizeof(T), s));
+        ozaki_prepare_ex(ctx->oz2, Bk, is_f32, 1, mp, nc_pad, mp, s);
+        done = ozaki_update_ex(ctx->oz2, G, is_f32, mp, mp, nc_pad, 1, 1.0, 0, 0, mp, 0, s) == 0;
+      }
+      if (!done) {
+        GemmArgs g{};
+        g.A = R; g.lda = mp; g.a_kmajor = 0;
+        g.B = Bk; g.ldb = mp; g.b_kmajor = 1;
+        g.C = G; g.ldc = mp; g.M = mp; g.N = nc_pad; g.K = mp;
+        launch_gemm<T>(g, s);
+      }
+      launch_vfe_cross_grad<T>(p.Zt, M, mp, p.Xt + c0 * D, nc, D, G, mp, rv, p.delta + c0, p.isn + c0, k->family, k->variance,
+                               k->linear_c, want_ard, nsplit, sums, qpart, upart, cap, zpart, s);
+      launch_vfe_point_grad<T>(qpart, upart, cap, nrb, nc, p.delta + c0, p.isn + c0, p.kd + c0, p.noise_v ? 1 : 0, p.noise_s,
+                               p.noise_v ? p.noise_v + c0 : nullptr, c, p.Xt + c0 * D, D, linear ? 1 : 0, k->linear_c,
+                               want_ard, sums, nm, nd ? nd + c0 : nullptr, md ? md + c0 : nullptr, s);
+    }
+    if (z_grad_out) {
+      launch_vfe_z_finish<T>(zpart, nsplit, mp, M, D, mult * k->variance, ard, layout, zz, zout, s);
+      int rc = download<T>(ctx, z_grad_out, zout, (size_t)M * D, false); if (rc) return rc;
+    }
+    { int rc = download<T>(ctx, noise_diag_out, nd, (size_t)N, false); if (rc) return rc; }
+    { int rc = download<T>(ctx, mean_diag_out, md, (size_t)N, false); if (rc) return rc; }
+    std::vector<double> h((size_t)nsums + 2);
+    std::vector<T> ard_h((size_t)(D > 0 ? D : 1));
+    CK(cudaMemcpyAsync(h.data(), sums, h.size() * sizeof(double), cudaMemcpyDeviceToHost, s));
+    if (want_ard) CK(cudaMemcpyAsync(ard_h.data(), p.ard, (size_t)D * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    CK(cudaGetLastError());
+    if (value_out) { const T v = (T)(objective == 0 ? p.elbo : p.dtc); memcpy(value_out, &v, sizeof(T)); }
+    if (!grad_out) return AGP_OK;
+    const double var = k->variance, sc_ = k->scale;  // the mapping of post_logpdf_grad_impl
+    grad_out[0] = 0.5 * h[0];
+    grad_out[1] = (k->transform == AGP_T_SCALE) ? (linear ? var * h[1] / sc_ : 0.5 * var * h[1] / sc_) : 0.0;
+    grad_out[2] = linear ? 0.5 * var * h[2] : 0.0;
+    grad_out[3] = h[(size_t)nsums];
+    grad_out[4] = h[(size_t)nsums + 1];
+    for (int d = 0; d < D; ++d)
+      grad_out[5 + d] = want_ard ? (linear ? var : 0.5 * var) * h[(size_t)5 + d] / (double)ard_h[(size_t)d] : 0.0;
+    return AGP_OK;
+  };
+  return vfe_core<T>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, nullptr, nullptr, nullptr, &grad);
+}
+
+// fp32 problems: the value is the fp32 pass's, the value agp_vfe_elbo returns; the gradient is formed in fp64 on the
+// same problem converted to fp64 (pass 1 included), because its adjoints are differences of terms up to ~1e5 times larger
+// than the result (agp.h).  Inputs and outputs keep the caller's memory space.
+int vfe_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout, const void* X,
+                 int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y, int objective,
+                 void* value_out, double* grad_out, void* noise_diag_out, void* mean_diag_out, void* z_grad_out) {
+  if (objective != 0 && objective != 1) { ctx->err = "objective must be 0 (elbo) or 1 (DTC)"; return AGP_ERR_INVALID; }
+  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
+  if (k && k->family == AGP_COMPOSITE) { ctx->err = "composite kernels are supported on the exact path only (not VFE)"; return AGP_ERR_UNSUPPORTED; }
+  if (ctx->nccl) { ctx->err = "the VFE gradient runs on a single-GPU context"; return AGP_ERR_UNSUPPORTED; }
+  int rc = check_kernel(ctx, k, D);
+  if (rc) return rc;
+  if (N <= 0 || M <= 0) { ctx->err = "N and M must be positive"; return AGP_ERR_DIM_MISMATCH; }
+  if (!X || !Zind || !y) { ctx->err = "X/Z/y is NULL"; return AGP_ERR_INVALID; }
+  if (value_out) {
+    float v[2];
+    rc = vfe_core<float>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, &v[0], &v[1], nullptr);
+    if (rc) return rc;
+    memcpy(value_out, &v[objective], sizeof(float));
+  }
+  cudaStream_t s = ctx->stream;
+  const bool dev = ctx->memspace == AGP_MEM_DEVICE;
+  auto widen = [](const void* v, int64_t n) {  // host-side parameter arrays (always host memory, agp.h)
+    std::vector<double> out((size_t)n);
+    for (int64_t i = 0; i < n; ++i) out[(size_t)i] = (double)((const float*)v)[i];
+    return out;
+  };
+  agp_kernel k64 = *k;
+  std::vector<double> ard64, mean64, noise64, jit64;
+  if (k->transform == AGP_T_ARD && k->ard) { ard64 = widen(k->ard, D); k64.ard = ard64.data(); }
+  agp_mean m64{};
+  agp_noise n64{}, j64{};
+  if (mean) { m64 = *mean; if (mean->kind == 2 && mean->v) { mean64 = widen(mean->v, N); m64.v = mean64.data(); } }
+  if (noise) { n64 = *noise; if (noise->kind == 1 && noise->v) { noise64 = widen(noise->v, N); n64.v = noise64.data(); } }
+  if (jitter) { j64 = *jitter; if (jitter->kind == 1 && jitter->v) { jit64 = widen(jitter->v, M); j64.v = jit64.data(); } }
+  // the point sets, the targets and the outputs: host vectors, or device buffers under AGP_MEM_DEVICE
+  Scratch sc(ctx);
+  std::vector<double> hX, hZ, hy, hnd, hmd, hz;
+  const void *X64, *Z64, *y64;
+  double *nd64 = nullptr, *md64 = nullptr, *z64 = nullptr;
+  if (!dev) {
+    hX = widen(X, N * D); hZ = widen(Zind, M * D); hy = widen(y, N);
+    X64 = hX.data(); Z64 = hZ.data(); y64 = hy.data();
+    if (noise_diag_out) { hnd.resize((size_t)N); nd64 = hnd.data(); }
+    if (mean_diag_out) { hmd.resize((size_t)N); md64 = hmd.data(); }
+    if (z_grad_out) { hz.resize((size_t)(M * D)); z64 = hz.data(); }
+  } else {
+    void* tmp = nullptr;
+    CK(sc.alloc(&tmp, (size_t)(N * D + M * D + N) * sizeof(double)));
+    double* b = (double*)tmp;
+    launch_cast<float, double>((const float*)X, b, N * D, s);
+    launch_cast<float, double>((const float*)Zind, b + N * D, M * D, s);
+    launch_cast<float, double>((const float*)y, b + N * D + M * D, N, s);
+    X64 = b; Z64 = b + N * D; y64 = b + N * D + M * D;
+    CK(sc.alloc(&tmp, (size_t)(2 * N + M * D) * sizeof(double)));
+    double* o = (double*)tmp;
+    if (noise_diag_out) nd64 = o;
+    if (mean_diag_out) md64 = o + N;
+    if (z_grad_out) z64 = o + 2 * N;
+  }
+  rc = vfe_grad_impl<double>(ctx, &k64, mean ? &m64 : nullptr, noise ? &n64 : nullptr, layout, X64, N, D, Z64, M,
+                             jitter ? &j64 : nullptr, y64, objective, nullptr, grad_out, nd64, md64, z64);
+  if (rc) return rc;
+  auto narrow = [&](const double* src, void* dst, int64_t n) -> int {
+    if (!dst) return AGP_OK;
+    if (!dev) {
+      for (int64_t i = 0; i < n; ++i) ((float*)dst)[i] = (float)src[i];
+      return AGP_OK;
+    }
+    launch_cast<double, float>(src, (float*)dst, n, s);
+    return AGP_OK;
+  };
+  narrow(nd64, noise_diag_out, N);
+  narrow(md64, mean_diag_out, N);
+  narrow(z64, z_grad_out, M * D);
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
   return AGP_OK;
 }
 
@@ -2670,6 +2920,17 @@ int32_t agp_vfe_elbo(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp
   if (!ctx) return AGP_ERR_INVALID;
   return DISPATCH(dtype, vfe_core<float>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, elbo_out, dtc_out, nullptr),
                   vfe_core<double>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, elbo_out, dtc_out, nullptr));
+}
+int32_t agp_vfe_elbo_grad(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
+                          int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,
+                          const agp_noise* jitter, const void* y, int32_t objective, void* value_out, double* grad_out,
+                          void* noise_diag_out, void* mean_diag_out, void* z_grad_out) {
+  if (!ctx) return AGP_ERR_INVALID;
+  return DISPATCH(dtype,
+                  vfe_grad_f32(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out, grad_out,
+                               noise_diag_out, mean_diag_out, z_grad_out),
+                  vfe_grad_impl<double>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out,
+                                        grad_out, noise_diag_out, mean_diag_out, z_grad_out));
 }
 int32_t agp_vfe_fit(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
                     int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,

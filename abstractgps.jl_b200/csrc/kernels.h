@@ -162,6 +162,29 @@ int64_t grad_x_part_len(int64_t n, int D, int nacc);
 template <typename T> void launch_grad_x(const T* X, int D, int64_t n, const T* Cinv, int64_t ldc, const T* alpha,
                                          const CompositeDesc& cd, double mult, const T* ard, int layout, double* part,
                                          T* out, cudaStream_t s);
+// gradient of the VFE objectives (vfe_grad.cu).  H = c I - Lam^-1 - m_e m_e', E = c D - I + Lam^-1 + m_e m_e' (m_pad x m_pad,
+// full, 0 outside M x M) from Lam^-1 (full), D = Lam - I (lower storage) and m_e
+template <typename T> void launch_vfe_hz(const T* Laminv, const T* Dl, int64_t ldd, const T* me, int64_t M, int64_t m_pad,
+                                         double c, T* H, T* E, cudaStream_t s);
+// row blocks and the column ranges of the inducing-point partials for chunks of up to `cap` points
+void vfe_cross_shape(int64_t m_pad, int64_t cap, int* nrb, int* nsplit);
+// one chunk: hyper-parameter sums (grad_reduce units, 5 + D), column sums q / u (qpart / upart: nrb rows of ldq) and the
+// inducing-point partials zpart (nsplit x D x m_pad, accumulated across chunks) from G = R K_zx,c (ldg) and r
+template <typename T> void launch_vfe_cross_grad(const T* Zt, int64_t M, int64_t m_pad, const T* Xc, int64_t nc, int D,
+                                                 const T* G, int64_t ldg, const T* r, const T* delta, const T* isn, int family,
+                                                 double variance, double linear_c, int want_ard, int nsplit, double* sums,
+                                                 double* qpart, double* upart, int64_t ldq, double* zpart, cudaStream_t s);
+// one chunk: noise / mean adjoints per point, their sums nm[0..1], and the kdiag term of the hyper-parameter sums
+template <typename T> void launch_vfe_point_grad(const double* qpart, const double* upart, int64_t ldq, int nrb, int64_t nc,
+                                                 const T* delta, const T* isn, const T* kd, int noise_kind, double noise_s,
+                                                 const T* noise_v, double c, const T* Xc, int D, int linear, double linear_c,
+                                                 int want_ard, double* sums, double* nm, T* noise_diag, T* mean_diag,
+                                                 cudaStream_t s);
+// out (M x D in `layout`) = zz + mult * chain_d * sum_q zpart[q]  (chain_d = ard[d], or 1 when ard is null)
+template <typename T> void launch_vfe_z_finish(const double* zpart, int nsplit, int64_t ldz, int64_t M, int D, double mult,
+                                               const T* ard, int layout, const T* zz, T* out, cudaStream_t s);
+// out[i] = (D)in[i]: the fp32 problems of the VFE gradient are converted to fp64 and back (vfe_grad.cu)
+template <typename S, typename D> void launch_cast(const S* in, D* out, int64_t n, cudaStream_t s);
 template <typename T> void launch_add_diag(T* A, int64_t lda, int64_t n, double v, cudaStream_t s);
 template <typename T> void launch_sumsq(const T* p, int64_t n, double* out, cudaStream_t s);  // out += sum p^2
 template <typename T> void launch_vfe_prep(const T* y, int64_t n, int mean_kind, double mean_c, const T* mean_v,

@@ -244,6 +244,37 @@ int32_t agp_vfe_elbo(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp
                      const agp_noise* noise, int32_t layout, const void* X, int64_t N, int32_t D,
                      const void* Zind, int64_t M, const agp_noise* jitter, const void* y,
                      void* elbo_out, void* dtc_out);
+/* Gradient of approx_log_evidence(VFE | DTC, fx, y), src/sparse_approximations.jl:248-254 / :282-286: what reverse-mode
+ * AD returns through the reference when a sparse GP is trained.  objective 0 = elbo, 1 = DTC.  With s_i = sigma_i^2,
+ * delta = s^-1/2 (y - m), K_zz + J = L_z L_z', A = L_z^-1 K_zx S^-1/2, Lam = I + A A', m_e = Lam^-1 A delta, V_z = L_z^-1
+ * and c = 1 (elbo) | 0 (DTC):
+ *   Kbar_zx = V_z' H V_z K_zx S^-1 + V_z' m_e (delta o s^-1/2)',  H = c I - Lam^-1 - m_e m_e'
+ *   Kbar_zz = -1/2 V_z' E V_z,  E = c (Lam - I) - I + Lam^-1 + m_e m_e';   kdiagbar_i = -c / (2 s_i)
+ *   d/d theta = sum Kbar_zz o dK_zz + sum Kbar_zx o dK_zx + sum kdiagbar o dkdiag
+ *   d/d z_m = 2 sum_m' Kbar_zz[m, m'] d1k(z_m, z_m') + sum_n Kbar_zx[m, n] d1k(z_m, x_n)
+ *   d/d s_i = -1/(2 s_i) + c kdiag_i/(2 s_i^2) - q_i/(2 s_i) - deltabar_i delta_i/(2 s_i),  d/d m_i = -s_i^-1/2 deltabar_i
+ *   with u = K_zx' V_z' m_e, q_i = sum_m Kbar_zx[m, i] K_zx[m, i], deltabar = -delta + s^-1/2 o u.
+ * value_out: 1 value of `dtype`, computed by the pass agp_vfe_elbo makes (for fp32 that fp32 pass itself); it agrees with
+ * agp_vfe_elbo's value to rounding, not bit for bit, because that pass sums its scalars with fp64 atomics.
+ * grad_out (double, 5 + D, NULL allowed): the layout of agp_post_logpdf_grad -- [3] is d/d sigma^2 of a scalar noise
+ * (the sum of the per-point derivatives), [4] d/d ConstMean c (the sum of the per-point ones).
+ * noise_diag_out / mean_diag_out: N values of `dtype` (d/d sigma_i^2, d/d m_i) or NULL.
+ * z_grad_out: M x D values of `dtype` in `layout` (AGP_POINT_MAJOR: D x M column-major, AGP_FEATURE_MAJOR: M x D
+ * column-major), with respect to the untransformed inducing points, or NULL; a DEVICE pointer under AGP_MEM_DEVICE, as are
+ * noise_diag_out and mean_diag_out.  Coincident points contribute 0 for the stationary families (agp_post_logpdf_grad_x).
+ * Single kernels only (the kernels agp_vfe_elbo accepts).  For AGP_F32 the gradient is formed in fp64 on the problem
+ * converted to fp64 (its own pass 1 included) and rounded to fp32 at the end: the adjoints are differences of terms up
+ * to ~1e5 times larger than the result, which fp32 arithmetic cannot carry.  G = R K_zx runs on the int8-slice product
+ * where pass 1's long-K product does (M >= 1024 under the automatic policy), on the tile GEMM otherwise.  The gradient
+ * with respect to X and to the jitter is not formed.
+ * Summed in fp64.  noise_diag_out, mean_diag_out and z_grad_out are summed in a fixed order (two calls give the same bits);
+ * the grad_out sums leave their CTAs through fp64 atomics, so two calls agree to rounding.  Errors: an objective other
+ * than 0 / 1 or a bad layout: AGP_ERR_INVALID; composite kernels and distributed contexts: AGP_ERR_UNSUPPORTED;
+ * K_zz + J or Lam not positive definite: AGP_ERR_NOT_POSDEF with agp_last_info, as agp_vfe_elbo. */
+int32_t agp_vfe_elbo_grad(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
+                          int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,
+                          const agp_noise* jitter, const void* y, int32_t objective, void* value_out, double* grad_out,
+                          void* noise_diag_out, void* mean_diag_out, void* z_grad_out);
 /* posterior(::VFE, fx, y) src/sparse_approximations.jl:58-75 */
 int32_t agp_vfe_fit(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean,
                     const agp_noise* noise, int32_t layout, const void* X, int64_t N, int32_t D,
