@@ -90,6 +90,8 @@ SIGNATURES = {
                                  _P, _P, _P]),
     "agp_vfe_elbo_grad": (C.c_int32, [_P, C.c_int32, _K, _M, _N, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _N,
                                       _P, C.c_int32, _P, C.POINTER(C.c_double), _P, _P, _P]),
+    "agp_vfe_elbo_grad_x": (C.c_int32, [_P, C.c_int32, _K, _M, _N, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64,
+                                        _N, _P, C.c_int32, _P, C.POINTER(C.c_double), _P, _P, _P, _P]),
     "agp_vfe_fit": (C.c_int32, [_P, C.c_int32, _K, _M, _N, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _N,
                                 _P, C.POINTER(_P)]),
     "agp_vfe_mean_var": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _P, _P]),

@@ -1265,12 +1265,17 @@ def elbo(vfe: VFE, fx: FiniteGP, y):
     return approx_log_evidence(vfe, fx, y)
 
 
-def approx_log_evidence_grad(vfe: VFE, fx: FiniteGP, y):
+def approx_log_evidence_grad(vfe: VFE, fx: FiniteGP, y, inputs=False):
     """(value, gradient dict) of approx_log_evidence(vfe, fx, y) -- the elbo for VFE, the DTC objective for DTC -- through
     one agp_vfe_elbo_grad call: what Zygote returns through the reference when a sparse GP is trained.  The dict has the
     keys of logpdf_grad ("variance", "scale" | "ard", "linear_c", "noise" scalar or per-point, "mean_c" | "mean_v") and
     "z", the gradient with respect to the inducing points, shaped like the container vfe.fz was built from (RowVecs: M x D,
-    ColVecs: D x M, a vector: length M) in the objective's dtype.  A CustomMean is treated as a constant of x."""
+    ColVecs: D x M, a vector: length M) in the objective's dtype.  A CustomMean is treated as a constant of x.
+
+    inputs=True also returns out["x"], the gradient with respect to the training inputs, shaped like the container fx was
+    built from (RowVecs: N x D, ColVecs: D x N, a vector: length N) in the objective's dtype; everything comes from one
+    agp_vfe_elbo_grad_x call.  A CustomMean and per-point noise are treated as constants of x: a caller whose mean or
+    noise depends on x chains through out["mean_v"] and out["noise"]."""
     eng = engine()
     f, dt, pts, z, y, ks, ms, ns, js, keep = _vfe_args(vfe, fx, y)
     D = pts.D
@@ -1286,10 +1291,15 @@ def approx_log_evidence_grad(vfe: VFE, fx: FiniteGP, y):
     zg = {"col": lambda: np.empty((D, z.n), dtype=dt, order="F"), "vec": lambda: np.empty(z.n, dtype=dt),
           "row": lambda: np.empty((z.n, D), dtype=dt)}[vfe.fz.x_kind]()
     objective = 1 if isinstance(vfe, DTC) else 0
-    eng.check(eng.L.agp_vfe_elbo_grad(eng.h, cabi.dtype_code(dt), C.byref(ks), C.byref(ms), C.byref(ns),
-                                      cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), pts.n, pts.D, cabi.ptr(z.a), z.n, C.byref(js),
-                                      cabi.ptr(y), objective, cabi.ptr(value), g.ctypes.data_as(C.POINTER(C.c_double)),
-                                      cabi.ptr(nd), cabi.ptr(md), cabi.ptr(zg)))
+    args = (eng.h, cabi.dtype_code(dt), C.byref(ks), C.byref(ms), C.byref(ns), cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), pts.n,
+            pts.D, cabi.ptr(z.a), z.n, C.byref(js), cabi.ptr(y), objective, cabi.ptr(value),
+            g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), cabi.ptr(md), cabi.ptr(zg))
+    if inputs:  # point-major like z: D x N column-major, i.e. N x D row-major
+        xg = {"col": lambda: np.empty((D, pts.n), dtype=dt, order="F"), "vec": lambda: np.empty(pts.n, dtype=dt),
+              "row": lambda: np.empty((pts.n, D), dtype=dt)}[fx.x_kind]()
+        eng.check(eng.L.agp_vfe_elbo_grad_x(*args, cabi.ptr(xg)))
+    else:
+        eng.check(eng.L.agp_vfe_elbo_grad(*args))
     out = {"variance": g[0]}
     if isinstance(k.transform, ScaleTransform):
         out["scale"] = g[1]
@@ -1303,14 +1313,16 @@ def approx_log_evidence_grad(vfe: VFE, fx: FiniteGP, y):
     elif isinstance(f.mean, CustomMean):
         out["mean_v"] = md.astype(np.float64)
     out["z"] = zg
+    if inputs:
+        out["x"] = xg
     return value[0], out
 
 
-def elbo_grad(vfe: VFE, fx: FiniteGP, y):
+def elbo_grad(vfe: VFE, fx: FiniteGP, y, inputs=False):
     """(elbo, gradient dict) of elbo(vfe::VFE, fx, y); VFE only, as elbo.  See approx_log_evidence_grad."""
     if isinstance(vfe, DTC):
         raise TypeError("elbo is defined for VFE; use approx_log_evidence for DTC")
-    return approx_log_evidence_grad(vfe, fx, y)
+    return approx_log_evidence_grad(vfe, fx, y, inputs=inputs)
 
 
 def _vfe_posterior(vfe: VFE, fx: FiniteGP, y):

@@ -1800,12 +1800,12 @@ int vfe_core(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
 // part goes through the exact path's reductions with alpha = 0 and C^-1 = P: grad_reduce_kernel gives
 // 1/2 sum (-P) o dK_zz = sum Kbar_zz o dK_zz, grad_x_kernel gives sum_m' (-P) d1k = 2 sum Kbar_zz d1k.  Pass 2 streams the
 // data in pass 1's chunks: K_zx,c by the Gram kernel, G = R K_zx,c by the tile GEMM, then vfe_cross_grad_kernel and
-// vfe_point_grad_kernel.
+// vfe_point_grad_kernel, and with x_grad_out vfe_x_grad_kernel and vfe_x_finish_kernel on the same G (vfe_grad_x.cu).
 template <typename T>
 int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout,
                   const void* X, int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y,
                   int objective, void* value_out, double* grad_out, void* noise_diag_out, void* mean_diag_out,
-                  void* z_grad_out) {
+                  void* z_grad_out, void* x_grad_out) {
   if (objective != 0 && objective != 1) { ctx->err = "objective must be 0 (elbo) or 1 (DTC)"; return AGP_ERR_INVALID; }
   if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
   if (k && k->family == AGP_COMPOSITE) { ctx->err = "composite kernels are supported on the exact path only (not VFE)"; return AGP_ERR_UNSUPPORTED; }
@@ -1879,6 +1879,18 @@ int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
     T *nd = nullptr, *md = nullptr;
     if (noise_diag_out) { CK(sc.alloc(&tmp, (size_t)N * sizeof(T))); nd = (T*)tmp; }
     if (mean_diag_out) { CK(sc.alloc(&tmp, (size_t)N * sizeof(T))); md = (T*)tmp; }
+    // the input gradient: per-chunk partials (row ranges x (D + 1) x cap), written in place under AGP_MEM_DEVICE
+    int xsplit = 0;
+    double* xpart = nullptr;
+    T* xout = nullptr;
+    const bool x_dev = ctx->memspace == AGP_MEM_DEVICE || ctx->out_dev_override;
+    if (x_grad_out) {
+      vfe_x_shape(mp, cap, &xsplit);
+      CK(sc.alloc(&tmp, (size_t)xsplit * (D + 1) * cap * sizeof(double)));
+      xpart = (double*)tmp;
+      if (x_dev) xout = (T*)x_grad_out;
+      else { CK(sc.alloc(&tmp, (size_t)N * D * sizeof(T))); xout = (T*)tmp; }
+    }
     for (int64_t c0 = 0; c0 < N; c0 += cap) {
       const int64_t nc = (N - c0 < cap) ? (N - c0) : cap;
       const int64_t nc_pad = round_up(nc, TILE);
@@ -1903,7 +1915,14 @@ int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
       launch_vfe_point_grad<T>(qpart, upart, cap, nrb, nc, p.delta + c0, p.isn + c0, p.kd + c0, p.noise_v ? 1 : 0, p.noise_s,
                                p.noise_v ? p.noise_v + c0 : nullptr, c, p.Xt + c0 * D, D, linear ? 1 : 0, k->linear_c,
                                want_ard, sums, nm, nd ? nd + c0 : nullptr, md ? md + c0 : nullptr, s);
+      if (x_grad_out) {
+        launch_vfe_x_grad<T>(p.Zt, M, mp, p.Xt + c0 * D, nc, D, G, mp, rv, p.delta + c0, p.isn + c0, k->family, xsplit, xpart,
+                             cap, s);
+        launch_vfe_x_finish<T>(xpart, xsplit, cap, nc, D, p.Xt + c0 * D, p.isn + c0, linear ? 1 : 0, k->variance, c, mult,
+                               ard, layout, N, c0, xout, s);
+      }
     }
+    if (x_grad_out && !x_dev) { int rc = download<T>(ctx, x_grad_out, xout, (size_t)N * D, false); if (rc) return rc; }
     if (z_grad_out) {
       launch_vfe_z_finish<T>(zpart, nsplit, mp, M, D, mult * k->variance, ard, layout, zz, zout, s);
       int rc = download<T>(ctx, z_grad_out, zout, (size_t)M * D, false); if (rc) return rc;
@@ -1936,7 +1955,8 @@ int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
 // than the result (agp.h).  Inputs and outputs keep the caller's memory space.
 int vfe_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout, const void* X,
                  int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y, int objective,
-                 void* value_out, double* grad_out, void* noise_diag_out, void* mean_diag_out, void* z_grad_out) {
+                 void* value_out, double* grad_out, void* noise_diag_out, void* mean_diag_out, void* z_grad_out,
+                 void* x_grad_out) {
   if (objective != 0 && objective != 1) { ctx->err = "objective must be 0 (elbo) or 1 (DTC)"; return AGP_ERR_INVALID; }
   if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
   if (k && k->family == AGP_COMPOSITE) { ctx->err = "composite kernels are supported on the exact path only (not VFE)"; return AGP_ERR_UNSUPPORTED; }
@@ -1968,15 +1988,16 @@ int vfe_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const 
   if (jitter) { j64 = *jitter; if (jitter->kind == 1 && jitter->v) { jit64 = widen(jitter->v, M); j64.v = jit64.data(); } }
   // the point sets, the targets and the outputs: host vectors, or device buffers under AGP_MEM_DEVICE
   Scratch sc(ctx);
-  std::vector<double> hX, hZ, hy, hnd, hmd, hz;
+  std::vector<double> hX, hZ, hy, hnd, hmd, hz, hx;
   const void *X64, *Z64, *y64;
-  double *nd64 = nullptr, *md64 = nullptr, *z64 = nullptr;
+  double *nd64 = nullptr, *md64 = nullptr, *z64 = nullptr, *x64 = nullptr;
   if (!dev) {
     hX = widen(X, N * D); hZ = widen(Zind, M * D); hy = widen(y, N);
     X64 = hX.data(); Z64 = hZ.data(); y64 = hy.data();
     if (noise_diag_out) { hnd.resize((size_t)N); nd64 = hnd.data(); }
     if (mean_diag_out) { hmd.resize((size_t)N); md64 = hmd.data(); }
     if (z_grad_out) { hz.resize((size_t)(M * D)); z64 = hz.data(); }
+    if (x_grad_out) { hx.resize((size_t)(N * D)); x64 = hx.data(); }
   } else {
     void* tmp = nullptr;
     CK(sc.alloc(&tmp, (size_t)(N * D + M * D + N) * sizeof(double)));
@@ -1990,9 +2011,10 @@ int vfe_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const 
     if (noise_diag_out) nd64 = o;
     if (mean_diag_out) md64 = o + N;
     if (z_grad_out) z64 = o + 2 * N;
+    if (x_grad_out) { CK(sc.alloc(&tmp, (size_t)N * D * sizeof(double))); x64 = (double*)tmp; }
   }
   rc = vfe_grad_impl<double>(ctx, &k64, mean ? &m64 : nullptr, noise ? &n64 : nullptr, layout, X64, N, D, Z64, M,
-                             jitter ? &j64 : nullptr, y64, objective, nullptr, grad_out, nd64, md64, z64);
+                             jitter ? &j64 : nullptr, y64, objective, nullptr, grad_out, nd64, md64, z64, x64);
   if (rc) return rc;
   auto narrow = [&](const double* src, void* dst, int64_t n) -> int {
     if (!dst) return AGP_OK;
@@ -2006,6 +2028,7 @@ int vfe_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const 
   narrow(nd64, noise_diag_out, N);
   narrow(md64, mean_diag_out, N);
   narrow(z64, z_grad_out, M * D);
+  narrow(x64, x_grad_out, N * D);
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
   return AGP_OK;
@@ -2921,16 +2944,23 @@ int32_t agp_vfe_elbo(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp
   return DISPATCH(dtype, vfe_core<float>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, elbo_out, dtc_out, nullptr),
                   vfe_core<double>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, elbo_out, dtc_out, nullptr));
 }
+int32_t agp_vfe_elbo_grad_x(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
+                            int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,
+                            const agp_noise* jitter, const void* y, int32_t objective, void* value_out, double* grad_out,
+                            void* noise_diag_out, void* mean_diag_out, void* z_grad_out, void* x_grad_out) {
+  if (!ctx) return AGP_ERR_INVALID;
+  return DISPATCH(dtype,
+                  vfe_grad_f32(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out, grad_out,
+                               noise_diag_out, mean_diag_out, z_grad_out, x_grad_out),
+                  vfe_grad_impl<double>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out,
+                                        grad_out, noise_diag_out, mean_diag_out, z_grad_out, x_grad_out));
+}
 int32_t agp_vfe_elbo_grad(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
                           int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,
                           const agp_noise* jitter, const void* y, int32_t objective, void* value_out, double* grad_out,
                           void* noise_diag_out, void* mean_diag_out, void* z_grad_out) {
-  if (!ctx) return AGP_ERR_INVALID;
-  return DISPATCH(dtype,
-                  vfe_grad_f32(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out, grad_out,
-                               noise_diag_out, mean_diag_out, z_grad_out),
-                  vfe_grad_impl<double>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out,
-                                        grad_out, noise_diag_out, mean_diag_out, z_grad_out));
+  return agp_vfe_elbo_grad_x(ctx, dtype, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out, grad_out,
+                             noise_diag_out, mean_diag_out, z_grad_out, nullptr);
 }
 int32_t agp_vfe_fit(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
                     int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,

@@ -183,6 +183,16 @@ template <typename T> void launch_vfe_point_grad(const double* qpart, const doub
 // out (M x D in `layout`) = zz + mult * chain_d * sum_q zpart[q]  (chain_d = ard[d], or 1 when ard is null)
 template <typename T> void launch_vfe_z_finish(const double* zpart, int nsplit, int64_t ldz, int64_t M, int D, double mult,
                                                const T* ard, int layout, const T* zz, T* out, cudaStream_t s);
+// gradient of the VFE objectives with respect to the training inputs (vfe_grad_x.cu): the row ranges of the partials for
+// chunks of up to `cap` points; one chunk's partials (nsplit x (D + 1) x ldx doubles, overwritten) from the same G and r
+// as launch_vfe_cross_grad; then out (N x D in `layout`, rows c0 .. c0 + nc) from them (c = 1 elbo | 0 DTC)
+void vfe_x_shape(int64_t m_pad, int64_t cap, int* nsplit);
+template <typename T> void launch_vfe_x_grad(const T* Zt, int64_t M, int64_t m_pad, const T* Xc, int64_t nc, int D,
+                                             const T* G, int64_t ldg, const T* r, const T* delta, const T* isn, int family,
+                                             int nsplit, double* xpart, int64_t ldx, cudaStream_t s);
+template <typename T> void launch_vfe_x_finish(const double* xpart, int nsplit, int64_t ldx, int64_t nc, int D, const T* Xc,
+                                               const T* isn, int linear, double variance, double c, double mult,
+                                               const T* ard, int layout, int64_t N, int64_t c0, T* out, cudaStream_t s);
 // out[i] = (D)in[i]: the fp32 problems of the VFE gradient are converted to fp64 and back (vfe_grad.cu)
 template <typename S, typename D> void launch_cast(const S* in, D* out, int64_t n, cudaStream_t s);
 template <typename T> void launch_add_diag(T* A, int64_t lda, int64_t n, double v, cudaStream_t s);

@@ -266,7 +266,7 @@ int32_t agp_vfe_elbo(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp
  * converted to fp64 (its own pass 1 included) and rounded to fp32 at the end: the adjoints are differences of terms up
  * to ~1e5 times larger than the result, which fp32 arithmetic cannot carry.  G = R K_zx runs on the int8-slice product
  * where pass 1's long-K product does (M >= 1024 under the automatic policy), on the tile GEMM otherwise.  The gradient
- * with respect to X and to the jitter is not formed.
+ * with respect to X is agp_vfe_elbo_grad_x's; the gradient with respect to the jitter is not formed.
  * Summed in fp64.  noise_diag_out, mean_diag_out and z_grad_out are summed in a fixed order (two calls give the same bits);
  * the grad_out sums leave their CTAs through fp64 atomics, so two calls agree to rounding.  Errors: an objective other
  * than 0 / 1 or a bad layout: AGP_ERR_INVALID; composite kernels and distributed contexts: AGP_ERR_UNSUPPORTED;
@@ -275,6 +275,25 @@ int32_t agp_vfe_elbo_grad(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, cons
                           int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,
                           const agp_noise* jitter, const void* y, int32_t objective, void* value_out, double* grad_out,
                           void* noise_diag_out, void* mean_diag_out, void* z_grad_out);
+/* The same outputs and, from the same passes, the gradient with respect to the training inputs X -- what reverse-mode AD
+ * returns for `x` through the reference's elbo, and what trains a feature network under a sparse GP
+ * (examples/2-deep-kernel-learning).  For data point n and input dimension d, with respect to the untransformed input:
+ *   x_grad[n, d] = sum_m Kbar_zx[m, n] dk(z_m, x_n)/dx_n[d] + kdiagbar_n dkdiag(x_n)/dx_n[d],   kdiagbar_n = -c / (2 s_n)
+ * With t the Scale s, the ARD v or 1 and x~ = t x:
+ *   SE / Matern   x_grad[n, d] = -sigma^2 t_d sum_m Kbar_zx[m, n] q(d2_mn) (z~_md - x~_nd),  q = kappa'(r) / r, the
+ *                 coefficient of z_grad's K_zx part with the opposite sign; coincident points contribute exactly 0 (for
+ *                 Matern 1/2 the zero subgradient); the kdiag term is 0
+ *   Linear        x_grad[n, d] = sigma^2 t_d (sum_m Kbar_zx[m, n] z~_md - c x~_nd / s_n)   (the second term is kdiag's)
+ * The mean and per-point noise are constants of X: the caller chains through mean_diag_out and noise_diag_out.
+ * x_grad_out: N x D values of `dtype` in `layout` (AGP_POINT_MAJOR: D x N column-major, AGP_FEATURE_MAJOR: N x D
+ * column-major), a DEVICE pointer under AGP_MEM_DEVICE; NULL: not computed.  Summed in fp64 in a fixed order (two calls
+ * give the same bits); the chunking of the data changes only the rounding.  Per chunk of the streamed pass it adds two
+ * launches (vfe_x_grad_kernel, vfe_x_finish_kernel); for AGP_F32 it is formed on the fp64 path like the rest and
+ * narrowed at the end.  Errors as agp_vfe_elbo_grad.  agp_vfe_elbo_grad(...) is agp_vfe_elbo_grad_x(..., NULL). */
+int32_t agp_vfe_elbo_grad_x(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
+                            int32_t layout, const void* X, int64_t N, int32_t D, const void* Zind, int64_t M,
+                            const agp_noise* jitter, const void* y, int32_t objective, void* value_out, double* grad_out,
+                            void* noise_diag_out, void* mean_diag_out, void* z_grad_out, void* x_grad_out);
 /* posterior(::VFE, fx, y) src/sparse_approximations.jl:58-75 */
 int32_t agp_vfe_fit(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean,
                     const agp_noise* noise, int32_t layout, const void* X, int64_t N, int32_t D,

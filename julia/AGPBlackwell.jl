@@ -545,10 +545,12 @@ function CRC.rrule(::typeof(logpdf), fx::DevFiniteGP{T}, y::AbstractVector{<:Rea
 end
 
 # ---- reverse-mode rules for the VFE objectives: elbo(VFE(fz), fx, y) and approx_log_evidence(VFE | DTC, fx, y) ---------
-# (src/sparse_approximations.jl:248-254, :282-286).  One agp_vfe_elbo_grad call returns the value, the kernel / noise /
+# (src/sparse_approximations.jl:248-254, :282-286).  One agp_vfe_elbo_grad_x call returns the value, the kernel / noise /
 # mean gradients in agp_post_logpdf_grad's layout (mapped back by the logpdf rule's helpers), the per-point noise and mean
-# gradients and the gradient with respect to the inducing points.  The kernel's tangent goes to fx.f (fz.f is the same
-# GP); fz receives the tangent of its inputs only, not of its jitter; fx.x receives none (agp.h).
+# gradients and the gradients with respect to the inducing points and the training inputs.  The kernel's tangent goes to
+# fx.f (fz.f is the same GP); fz receives the tangent of its inputs only, not of its jitter; fx.x receives the tangent of
+# its inputs, so a feature network that computes x learns from the GP term (the mean and per-point noise are taken as
+# constants of x, agp.h).
 z_storage(z::ColVecs, zg, layout) = layout == AGP_POINT_MAJOR ? zg : permutedims(zg)
 z_storage(z::RowVecs, zg, layout) = layout == AGP_FEATURE_MAJOR ? zg : permutedims(zg)
 z_storage(z::AbstractVector{<:Real}, zg, layout) = zg
@@ -560,19 +562,20 @@ function sparse_gradients(fz::FiniteGP, fx::DevFiniteGP{T}, y::AbstractVector{<:
     ks, k1 = kernel_spec(fx.f.kernel, T); ms, k2 = mean_spec(fx.f.mean, fx.x, T)
     ns, k3 = noise_spec(fx.Σy, T); js, k4 = noise_spec(fz.Σy, T)
     yv = convert(Vector{T}, y); val = Vector{T}(undef, 1); g = Vector{Float64}(undef, 5 + D)
-    nd = Vector{T}(undef, length(fx)); md = Vector{T}(undef, length(fx)); zg = similar(Z, T)
+    nd = Vector{T}(undef, length(fx)); md = Vector{T}(undef, length(fx)); zg = similar(Z, T); xg = similar(X, T)
     lock(c.lock) do
-        GC.@preserve X Z yv val g nd md zg k1 k2 k3 k4 check(c, ccall((:agp_vfe_elbo_grad, libagp), Int32,
+        GC.@preserve X Z yv val g nd md zg xg k1 k2 k3 k4 check(c, ccall((:agp_vfe_elbo_grad_x, libagp), Int32,
             (Ptr{Cvoid}, Int32, Ref{AgpKernel}, Ref{AgpMean}, Ref{AgpNoise}, Int32, Ptr{Cvoid}, Int64, Int32, Ptr{Cvoid}, Int64,
-             Ref{AgpNoise}, Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
-            c.h, agp_dtype(T), ks, ms, ns, layout, X, length(fx), D, Z, length(fz), js, yv, Int32(objective), val, g, nd, md, zg))
+             Ref{AgpNoise}, Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+            c.h, agp_dtype(T), ks, ms, ns, layout, X, length(fx), D, Z, length(fz), js, yv, Int32(objective), val, g, nd, md, zg,
+            xg))
     end
-    return val[1], g, nd, md, z_storage(fz.x, zg, layout)
+    return val[1], g, nd, md, z_storage(fz.x, zg, layout), xg
 end
 
 function vfe_rrule(approx, fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T}
     fz = approx.fz
-    val, gv, nd, md, zg = sparse_gradients(fz, fx, y, approx isa DTC ? 1 : 0)
+    val, gv, nd, md, zg, xg = sparse_gradients(fz, fx, y, approx isa DTC ? 1 : 0)
     g = (variance=gv[1], scale=gv[2], linear_c=gv[3], noise=gv[4], mean_c=gv[5], ard=gv[6:end], noise_diag=nd)
     _, var, _, w = flat(fx.f.kernel)
     w === nothing && (w = 1.0)
@@ -580,7 +583,7 @@ function vfe_rrule(approx, fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where 
         d = CRC.unthunk(Δ)
         gs = map(v -> v isa Number ? d * v : d .* v, g)
         f̄ = CRC.Tangent{typeof(fx.f)}(; mean=mean_tangent(fx.f.mean, gs), kernel=kernel_tangent(fx.f.kernel, gs, var, w))
-        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, Σy=noise_tangent(fx.Σy, gs))
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, d .* xg), Σy=noise_tangent(fx.Σy, gs))
         t_approx = CRC.Tangent{typeof(approx)}(; fz=CRC.Tangent{typeof(fz)}(; x=x_tangent(fz.x, d .* zg)))
         return CRC.NoTangent(), t_approx, f̄x, -d .* md                    # d/d y = -d/d m
     end
