@@ -86,6 +86,8 @@ SIGNATURES = {
     "agp_post_extend": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _P, _M, _N, _P, C.POINTER(_P)]),
     "agp_post_free": (C.c_int32, [_P]),
     "agp_rand": (C.c_int32, [_P, C.c_int32, _K, _M, _N, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P]),
+    "agp_rand_grad": (C.c_int32, [_P, C.c_int32, _K, _M, _N, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int32, _P,
+                                  C.POINTER(C.c_double), _P, _P, _P, _P]),
     "agp_vfe_elbo": (C.c_int32, [_P, C.c_int32, _K, _M, _N, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _N,
                                  _P, _P, _P]),
     "agp_vfe_elbo_grad": (C.c_int32, [_P, C.c_int32, _K, _M, _N, C.c_int32, _P, C.c_int64, C.c_int32, _P, C.c_int64, _N,

@@ -1168,6 +1168,70 @@ def rand_from_normals(fx: FiniteGP, Z, squeeze=False):
     return out[:, 0] if squeeze else out
 
 
+def rand_grad(fx: FiniteGP, Z, out_bar, inputs=False):
+    """(out, gradient dict) of out = rand_from_normals(fx, Z) = m + C.U' Z over a prior GP, pulled back from the cotangent
+    out_bar (the shape of Z: length N or N x S) -- what Zygote returns through the reference's rand(rng, fx, S)
+    (test/finite_gp_projection.jl:105-127) for reparameterised Monte Carlo objectives.  The gradient comes from one
+    agp_rand_grad call.  The dict has the keys of logpdf_grad ("kernel" for a composite, else "variance", "scale" | "ard",
+    "linear_c"; "noise" scalar or per-point; "mean_c" | "mean_v") and "Z", the cotangent of the normals, shaped like Z.
+    inputs=True also returns out["x"], the gradient with respect to the input points, shaped like the container fx was
+    built from (RowVecs: N x D, ColVecs: D x N, a vector: length N).  A CustomMean is treated as a constant of x: the
+    caller chains through out["mean_v"]."""
+    if not isinstance(fx.f, GP):
+        raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "the gradient of rand is implemented for a FiniteGP over a prior GP, not "
+                       "over %s" % type(fx.f).__name__)
+    eng = engine()
+    f = fx.f
+    dt = fx.dtype
+    pts = fx.x.astype(dt)
+    N, D = pts.n, pts.D
+    Zin = np.asarray(Z)
+    Zf = np.asfortranarray(np.asarray(Z, dtype=dt).reshape(N, -1))
+    Of = np.asfortranarray(np.asarray(out_bar, dtype=dt).reshape(N, -1))
+    if Of.shape != Zf.shape:
+        raise DimensionMismatch("out_bar has shape %s, Z has %s" % (np.shape(out_bar), Zin.shape))
+    S = Zf.shape[1]
+    out = rand_from_normals(fx, Zf)
+    keep = []
+    ks = _kernel_struct(f.kernel, dt, keep, D=D)
+    ms = _mean_struct(f.mean.spec(pts, dt), keep)
+    ns = _noise_struct(fx.s2, N, dt, keep)
+    k = f.kernel
+    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
+    flat = _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D) if composite else None
+    g = np.zeros(flat.grad_len() if composite else 5 + D, dtype=np.float64)
+    per_point = np.ndim(fx.s2) != 0
+    nd = np.empty(N, dtype=dt) if per_point else None
+    md = np.empty(N, dtype=dt) if isinstance(f.mean, CustomMean) else None
+    zb = np.empty((N, S), dtype=dt, order="F")
+    # the points go in point-major, so x comes back point-major: D x N column-major, i.e. N x D row-major
+    xg = {"col": lambda: np.empty((D, N), dtype=dt, order="F"), "vec": lambda: np.empty(N, dtype=dt),
+          "row": lambda: np.empty((N, D), dtype=dt)}[fx.x_kind]() if inputs else None
+    eng.check(eng.L.agp_rand_grad(eng.h, cabi.dtype_code(dt), C.byref(ks), C.byref(ms), C.byref(ns), cabi.AGP_POINT_MAJOR,
+                                  cabi.ptr(pts.a), N, D, cabi.ptr(Zf), S, cabi.ptr(Of),
+                                  g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), cabi.ptr(md), cabi.ptr(xg),
+                                  cabi.ptr(zb)))
+    if composite:
+        res = {"kernel": flat.params_grad(g)}
+    else:
+        res = {"variance": g[0]}
+        if isinstance(k.transform, ScaleTransform):
+            res["scale"] = g[1]
+        elif isinstance(k.transform, ARDTransform):
+            res["ard"] = g[5:5 + D].copy()
+        if k.family == LINEAR:
+            res["linear_c"] = g[2]
+    res["noise"] = nd.astype(np.float64) if per_point else g[3]
+    if isinstance(f.mean, ConstMean):
+        res["mean_c"] = g[4]
+    elif isinstance(f.mean, CustomMean):
+        res["mean_v"] = md.astype(np.float64)
+    res["Z"] = zb.reshape(Zin.shape) if Zin.ndim == 1 else zb
+    if inputs:
+        res["x"] = xg
+    return (out[:, 0] if Zin.ndim == 1 else out), res
+
+
 def _posterior_sequential(fx: FiniteGP, y):
     p: PosteriorGP = fx.f
     eng = engine()

@@ -1210,49 +1210,35 @@ static CompositeDesc single_kernel_desc(int family, double variance, double line
   return one;
 }
 
+// The reductions that end every gradient of this form, on the handle's points and kernel: with W = alpha alpha' - Cinv
+// (Cinv: its lower tiles are read, leading dimension n_pad),
+//   grad_out = the agp_post_logpdf_grad layout of 1/2 sum_ij W_ij dC_ij/dtheta ([3] = 1/2 tr W, [4] = sum alpha),
+//   noise_diag_out = 1/2 W_ii,  x_grad_out = sum_j W_ij d1k(x_i, x_j)  (agp_post_logpdf_grad_x).
+// Any output may be NULL.  agp_post_logpdf_grad_x runs it with C^-1; agp_rand_grad with alpha = 0 and Cinv = -V'QV.
 template <typename T>
-int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, int layout, void* x_grad_out) {
+int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, double* grad_out, void* noise_diag_out, int layout,
+                    void* x_grad_out) {
   agp_ctx* ctx = p->ctx;
-  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
-  { int rrc = post_replicate<T>(p); if (rrc) return rrc; }
   cudaStream_t s = ctx->stream;
-  CK(cudaSetDevice(ctx->device));
-  if (p->valid || p->segs.size() > 1) { ctx->err = "gradient of an extended (sequentially conditioned) posterior is unsupported"; return AGP_ERR_UNSUPPORTED; }
   const int64_t n = p->n, n_pad = p->n_pad;
   const int D = p->D;
   const bool want_theta = grad_out || noise_diag_out;  // the hyper-parameter reduction also yields noise_diag
-  if (!want_theta && !x_grad_out) return AGP_OK;
-  Scratch sc(ctx);
   void* tmp = nullptr;
-  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
-  T* V = (T*)tmp;
-  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
-  T* Cinv = (T*)tmp;
   const int64_t nsums = agp_post_grad_len(p);  // 5 + D for a single kernel
   CK(sc.alloc(&tmp, (size_t)nsums * sizeof(double)));
   double* sums = (double*)tmp;
   T* noise_d = nullptr;
   if (noise_diag_out) { CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T))); noise_d = (T*)tmp; }
-  CK(cudaMemsetAsync(V, 0, (size_t)n_pad * n_pad * sizeof(T), s));
   CK(cudaMemsetAsync(sums, 0, (size_t)nsums * sizeof(double), s));
-  launch_add_diag<T>(V, n_pad, n_pad, 1.0, s);
-  forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, V, n_pad, n_pad);
-  {
-    GemmArgs g{};  // C^-1 = V'V, lower tiles
-    g.A = V; g.lda = n_pad; g.a_kmajor = 1;
-    g.B = V; g.ldb = n_pad; g.b_kmajor = 1;
-    g.C = Cinv; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = 1;
-    launch_gemm<T>(g, s);
-  }
   const int want_ard = (p->k.transform == AGP_T_ARD) ? 1 : 0;
   if (want_theta) {
     if (p->comp)
-      launch_composite_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->comp->desc, sums, noise_d, s);
+      launch_composite_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, alpha, p->comp->desc, sums, noise_d, s);
     else
-      launch_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, (const T*)p->alpha, p->k.family, p->k.linear_c, want_ard,
+      launch_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, alpha, p->k.family, p->k.linear_c, want_ard,
                             sums, noise_d, s);
   }
-  if (x_grad_out) {  // sum_j W_ij d1k(x_i, x_j) from the same C^-1 (grad_x.cu)
+  if (x_grad_out) {  // sum_j W_ij d1k(x_i, x_j) from the same W (grad_x.cu)
     const CompositeDesc one = single_kernel_desc(p->k.family, p->k.variance, p->k.linear_c);
     const CompositeDesc* cd = &one;
     double mult = 1.0;
@@ -1267,7 +1253,7 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, i
     double* part = (double*)tmp;
     CK(sc.alloc(&tmp, (size_t)n * D * sizeof(T)));
     T* xg = (T*)tmp;
-    launch_grad_x<T>((const T*)p->Xt, D, n, Cinv, n_pad, (const T*)p->alpha, *cd, mult, ard, layout, part, xg, s);
+    launch_grad_x<T>((const T*)p->Xt, D, n, Cinv, n_pad, alpha, *cd, mult, ard, layout, part, xg, s);
     int rc = download<T>(ctx, x_grad_out, xg, (size_t)n * D, false); if (rc) return rc;
   }
   if (!want_theta) {
@@ -1305,6 +1291,36 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, i
   for (int d = 0; d < D; ++d)
     grad_out[5 + d] = want_ard ? (linear ? var : 0.5 * var) * h[(size_t)5 + d] / (double)ard_h[(size_t)d] : 0.0;
   return AGP_OK;
+}
+
+
+template <typename T>
+int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, int layout, void* x_grad_out) {
+  agp_ctx* ctx = p->ctx;
+  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
+  { int rrc = post_replicate<T>(p); if (rrc) return rrc; }
+  cudaStream_t s = ctx->stream;
+  CK(cudaSetDevice(ctx->device));
+  if (p->valid || p->segs.size() > 1) { ctx->err = "gradient of an extended (sequentially conditioned) posterior is unsupported"; return AGP_ERR_UNSUPPORTED; }
+  const int64_t n_pad = p->n_pad;
+  if (!grad_out && !noise_diag_out && !x_grad_out) return AGP_OK;
+  Scratch sc(ctx);
+  void* tmp = nullptr;
+  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
+  T* V = (T*)tmp;
+  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
+  T* Cinv = (T*)tmp;
+  CK(cudaMemsetAsync(V, 0, (size_t)n_pad * n_pad * sizeof(T), s));
+  launch_add_diag<T>(V, n_pad, n_pad, 1.0, s);
+  forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, V, n_pad, n_pad);
+  {
+    GemmArgs g{};  // C^-1 = V'V, lower tiles
+    g.A = V; g.lda = n_pad; g.a_kmajor = 1;
+    g.B = V; g.ldb = n_pad; g.b_kmajor = 1;
+    g.C = Cinv; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = 1;
+    launch_gemm<T>(g, s);
+  }
+  return grad_reductions<T>(p, sc, Cinv, (const T*)p->alpha, grad_out, noise_diag_out, layout, x_grad_out);
 }
 
 template <typename T>
@@ -1550,6 +1566,194 @@ int rand_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp
   launch_add_mean_cols<T>(Od, n_pad, N, S, mean->kind, mean->c, mean_d, s);
   cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   CK(cudaMemcpy2DAsync(out, (size_t)N * sizeof(T), Od, (size_t)n_pad * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kout, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return AGP_OK;
+}
+
+// ---- pullback of rand: out = m + L Z, C = K + Sigma_y = L L' (agp.h agp_rand_grad).  In fp64 whatever the caller's dtype
+// (rand_grad_f32).  The factor comes from the factor-only fit as an agp_post, so the reductions of the logpdf gradient
+// (grad_reductions) run on it with alpha = 0 and Cinv = -V'QV:
+//   Zbar = L' Obar;  Q = the lower triangle of Zbar Z' mirrored;  V = L^-1;  W1 = Q V;  -V' W1 into lower tiles.
+// Three n_pad x n_pad buffers besides the factor; ~4 N^3 flop (the substitution N^3, Q V 2 N^3, the lower half of V'W1 N^3).
+int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout, const void* X,
+                  int64_t N, int D, const void* Z, int S, const void* out_bar, double* grad_out, void* noise_diag_out,
+                  void* mean_diag_out, void* x_grad_out, void* z_bar_out) {
+  using T = double;
+  agp_post* p = nullptr;
+  int rc = fit_impl<T>(ctx, k, mean, noise, layout, X, N, D, nullptr, 0, nullptr, nullptr, &p, nullptr, nullptr, nullptr);
+  if (rc) return rc;
+  struct Guard { agp_post* p; ~Guard() { if (p) agp_post_free(p); } } guard{p};
+  cudaStream_t s = ctx->stream;
+  const int64_t n_pad = p->n_pad, s_pad = round_up(S, 4);
+  Scratch sc(ctx);
+  void* tmp = nullptr;
+  // the three N x N buffers first (fit_impl's note on the stream-ordered pool)
+  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
+  T* B1 = (T*)tmp;  // L', then W1 = Q V
+  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
+  T* B2 = (T*)tmp;  // Q, then -V'QV (lower tiles)
+  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
+  T* V = (T*)tmp;
+  CK(sc.alloc(&tmp, (size_t)n_pad * s_pad * sizeof(T) * 3));
+  T* Od = (T*)tmp; T* Zd = Od + n_pad * s_pad; T* Zb = Zd + n_pad * s_pad;
+  CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T)));
+  T* zero_alpha = (T*)tmp;
+  CK(sc.alloc(&tmp, (size_t)N * sizeof(double)));
+  double* mbar = (double*)tmp;
+  CK(cudaMemsetAsync(zero_alpha, 0, (size_t)n_pad * sizeof(T), s));
+  CK(cudaMemsetAsync(Od, 0, (size_t)n_pad * s_pad * sizeof(T) * 2, s));  // zero padding rows / columns of Obar and Z
+  const cudaMemcpyKind kin = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  if (S > 0) {
+    CK(cudaMemcpy2DAsync(Od, (size_t)n_pad * sizeof(T), out_bar, (size_t)N * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kin, s));
+    CK(cudaMemcpy2DAsync(Zd, (size_t)n_pad * sizeof(T), Z, (size_t)N * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kin, s));
+  }
+  // mbar_i = sum_s Obar_is
+  launch_rowsum<T>(Od, n_pad, N, S, mbar, s);
+  // Zbar = L' Obar: L' taken whole from the factor (its storage above the diagonal blocks is not zeroed)
+  launch_export_upper<T>((const T*)p->L, p->lda, n_pad, B1, n_pad, s);
+  {
+    GemmArgs g{};
+    g.A = B1; g.lda = n_pad; g.a_kmajor = 0;
+    g.B = Od; g.ldb = n_pad; g.b_kmajor = 1;
+    g.C = Zb; g.ldc = n_pad; g.M = n_pad; g.N = s_pad; g.K = n_pad;
+    launch_gemm<T>(g, s);
+  }
+  if (z_bar_out && S > 0)
+    CK(cudaMemcpy2DAsync(z_bar_out, (size_t)N * sizeof(T), Zb, (size_t)n_pad * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kout, s));
+  const bool want_c = grad_out || noise_diag_out || x_grad_out;
+  if (want_c) {
+    {
+      GemmArgs g{};  // Q = Zbar Z', lower tiles (K = S), then mirrored
+      g.A = Zb; g.lda = n_pad; g.a_kmajor = 0;
+      g.B = Zd; g.ldb = n_pad; g.b_kmajor = 0;
+      g.C = B2; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = s_pad; g.lower_only = 1;
+      launch_gemm<T>(g, s);
+      launch_symmetrize_lower<T>(B2, n_pad, n_pad, s);
+    }
+    CK(cudaMemsetAsync(V, 0, (size_t)n_pad * n_pad * sizeof(T), s));
+    launch_add_diag<T>(V, n_pad, n_pad, 1.0, s);
+    forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, V, n_pad, n_pad);
+    {
+      GemmArgs g{};  // W1 = Q V
+      g.A = B2; g.lda = n_pad; g.a_kmajor = 0;
+      g.B = V; g.ldb = n_pad; g.b_kmajor = 1;
+      g.C = B1; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad;
+      launch_gemm<T>(g, s);
+    }
+    {
+      GemmArgs g{};  // -V' W1 = -2 Cbar, lower tiles
+      g.A = V; g.lda = n_pad; g.a_kmajor = 1;
+      g.B = B1; g.ldb = n_pad; g.b_kmajor = 1;
+      g.C = B2; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = 1; g.alpha_neg = 1;
+      launch_gemm<T>(g, s);
+    }
+    rc = grad_reductions<T>(p, sc, B2, zero_alpha, grad_out, noise_diag_out, layout, x_grad_out);
+    if (rc) return rc;
+  }
+  rc = download<T>(ctx, mean_diag_out, mbar, (size_t)N, false);
+  if (rc) return rc;
+  if (grad_out) {  // d/d ConstMean c = sum_i mbar_i, in index order
+    std::vector<double> h((size_t)N);
+    CK(cudaMemcpyAsync(h.data(), mbar, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    double c = 0.0;
+    for (int64_t i = 0; i < N; ++i) c += h[(size_t)i];
+    grad_out[4] = c;
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return AGP_OK;
+}
+
+int rand_grad_check(agp_ctx* ctx, int layout, const void* X, const void* Z, int S, const void* out_bar) {
+  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
+  if (!X) { ctx->err = "X is NULL"; return AGP_ERR_INVALID; }
+  if (S < 0) { ctx->err = "S must be >= 0"; return AGP_ERR_INVALID; }
+  if (S > 0 && (!Z || !out_bar)) { ctx->err = "Z/out_bar is NULL"; return AGP_ERR_INVALID; }
+  if (ctx->nccl) { ctx->err = "the gradient of rand runs on a single-GPU context"; return AGP_ERR_UNSUPPORTED; }
+  return AGP_OK;
+}
+
+// fp32 problems: the pullback is formed on the problem converted to fp64 and its outputs rounded to fp32.  -V'QV carries
+// terms of the order of cond(C) that cancel (agp.h).  Parameter arrays are host memory (widened here); X, Z, out_bar and
+// the array outputs keep the caller's memory space.
+int rand_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout, const void* X,
+                  int64_t N, int D, const void* Z, int S, const void* out_bar, double* grad_out, void* noise_diag_out,
+                  void* mean_diag_out, void* x_grad_out, void* z_bar_out) {
+  int rc = check_kernel(ctx, k, D);
+  if (rc) return rc;
+  if (N <= 0) { ctx->err = "N must be positive"; return AGP_ERR_DIM_MISMATCH; }
+  cudaStream_t s = ctx->stream;
+  CK(cudaSetDevice(ctx->device));
+  const bool dev = ctx->memspace == AGP_MEM_DEVICE;
+  std::vector<std::vector<double>> keep;  // widened host arrays, alive for the call
+  auto widen = [&](const void* v, int64_t n) -> const double* {
+    if (!v) return nullptr;
+    keep.emplace_back((size_t)n);
+    for (int64_t i = 0; i < n; ++i) keep.back()[(size_t)i] = (double)((const float*)v)[i];
+    return keep.back().data();
+  };
+  agp_kernel k64 = *k;
+  agp_kernel_composite c64{};
+  std::vector<agp_kernel_factor> f64;
+  if (k->family == AGP_COMPOSITE && k->composite) {
+    c64 = *k->composite;
+    int nf = 0;
+    if (c64.nfactors && c64.nterms > 0 && c64.nterms <= AGP_COMP_MAX)
+      for (int t = 0; t < c64.nterms; ++t) nf += c64.nfactors[t] > 0 ? c64.nfactors[t] : 0;
+    if (c64.factors && nf <= AGP_COMP_MAX) {  // out-of-range descriptors are reported by comp_build
+      f64.assign(c64.factors, c64.factors + nf);
+      for (auto& f : f64) { f.ard = widen(f.ard, D); f.r = widen(f.r, D); }
+      c64.factors = f64.data();
+    }
+    k64.composite = &c64;
+  } else if (k->transform == AGP_T_ARD) {
+    k64.ard = widen(k->ard, D);
+  }
+  agp_mean m64{};
+  agp_noise n64{};
+  if (mean) { m64 = *mean; if (mean->kind == 2) m64.v = widen(mean->v, N); }
+  if (noise) { n64 = *noise; if (noise->kind == 1) n64.v = widen(noise->v, N); }
+  Scratch sc(ctx);
+  const double *X64 = nullptr, *Z64 = nullptr, *O64 = nullptr;
+  double *nd64 = nullptr, *md64 = nullptr, *x64 = nullptr, *zb64 = nullptr;
+  std::vector<double> hnd, hmd, hx, hzb;
+  const int64_t NS = N * (int64_t)S;
+  if (!dev) {
+    X64 = widen(X, N * D); Z64 = widen(Z, NS); O64 = widen(out_bar, NS);
+    if (noise_diag_out) { hnd.resize((size_t)N); nd64 = hnd.data(); }
+    if (mean_diag_out) { hmd.resize((size_t)N); md64 = hmd.data(); }
+    if (x_grad_out) { hx.resize((size_t)(N * D)); x64 = hx.data(); }
+    if (z_bar_out) { hzb.resize((size_t)NS); zb64 = hzb.data(); }
+  } else {
+    void* tmp = nullptr;
+    CK(sc.alloc(&tmp, (size_t)(N * D + 2 * NS) * sizeof(double)));
+    double* b = (double*)tmp;
+    launch_cast<float, double>((const float*)X, b, N * D, s);
+    X64 = b;
+    if (Z) { launch_cast<float, double>((const float*)Z, b + N * D, NS, s); Z64 = b + N * D; }
+    if (out_bar) { launch_cast<float, double>((const float*)out_bar, b + N * D + NS, NS, s); O64 = b + N * D + NS; }
+    CK(sc.alloc(&tmp, (size_t)(2 * N + N * D + NS) * sizeof(double)));
+    double* o = (double*)tmp;
+    if (noise_diag_out) nd64 = o;
+    if (mean_diag_out) md64 = o + N;
+    if (x_grad_out) x64 = o + 2 * N;
+    if (z_bar_out) zb64 = o + 2 * N + N * D;
+  }
+  rc = rand_grad_f64(ctx, &k64, mean ? &m64 : nullptr, noise ? &n64 : nullptr, layout, X64, N, D, Z64, S, O64, grad_out, nd64,
+                     md64, x64, zb64);
+  if (rc) return rc;
+  auto narrow = [&](const double* src, void* dst, int64_t n) {
+    if (!dst || n <= 0) return;
+    if (!dev) { for (int64_t i = 0; i < n; ++i) ((float*)dst)[i] = (float)src[i]; return; }
+    launch_cast<double, float>(src, (float*)dst, n, s);
+  };
+  narrow(nd64, noise_diag_out, N);
+  narrow(md64, mean_diag_out, N);
+  narrow(x64, x_grad_out, N * D);
+  narrow(zb64, z_bar_out, NS);
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
   return AGP_OK;
@@ -2842,6 +3046,18 @@ int32_t agp_rand(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mea
   if (!ctx) return AGP_ERR_INVALID;
   return DISPATCH(dtype, rand_impl<float>(ctx, k, mean, noise, layout, X, N, D, Z, S, out),
                   rand_impl<double>(ctx, k, mean, noise, layout, X, N, D, Z, S, out));
+}
+
+int32_t agp_rand_grad(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
+                      int32_t layout, const void* X, int64_t N, int32_t D, const void* Z, int32_t S, const void* out_bar,
+                      double* grad_out, void* noise_diag_out, void* mean_diag_out, void* x_grad_out, void* z_bar_out) {
+  if (!ctx) return AGP_ERR_INVALID;
+  int rc = rand_grad_check(ctx, layout, X, Z, S, out_bar);
+  if (rc) return rc;
+  return DISPATCH(dtype, rand_grad_f32(ctx, k, mean, noise, layout, X, N, D, Z, S, out_bar, grad_out, noise_diag_out,
+                                       mean_diag_out, x_grad_out, z_bar_out),
+                  rand_grad_f64(ctx, k, mean, noise, layout, X, N, D, Z, S, out_bar, grad_out, noise_diag_out,
+                                mean_diag_out, x_grad_out, z_bar_out));
 }
 
 int32_t agp_debug_ozaki_syrk(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* P_dev, int64_t lda, int64_t M, int64_t N,

@@ -196,6 +196,10 @@ template <typename T> void launch_vfe_x_finish(const double* xpart, int nsplit, 
 // out[i] = (D)in[i]: the fp32 problems of the VFE gradient are converted to fp64 and back (vfe_grad.cu)
 template <typename S, typename D> void launch_cast(const S* in, D* out, int64_t n, cudaStream_t s);
 template <typename T> void launch_add_diag(T* A, int64_t lda, int64_t n, double v, cudaStream_t s);
+// pullback of rand (rand_grad.cu): A(i, j) = A(j, i) for i < j < n (the strict lower triangle copied onto the upper one),
+// and out[i] = sum_{s < S} A[i + s*lda] in fp64, in order
+template <typename T> void launch_symmetrize_lower(T* A, int64_t lda, int64_t n, cudaStream_t s);
+template <typename T> void launch_rowsum(const T* A, int64_t lda, int64_t n, int S, double* out, cudaStream_t s);
 template <typename T> void launch_sumsq(const T* p, int64_t n, double* out, cudaStream_t s);  // out += sum p^2
 template <typename T> void launch_vfe_prep(const T* y, int64_t n, int mean_kind, double mean_c, const T* mean_v,
                                            int noise_kind, double noise_s, const T* noise_v, const T* kdiag,

@@ -235,6 +235,37 @@ int32_t agp_post_free(agp_post* p);
 int32_t agp_rand(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean,
                  const agp_noise* noise, int32_t layout, const void* X, int64_t N, int32_t D,
                  const void* Z, int32_t S, void* out);
+/* Pullback of agp_rand at the same arguments: what reverse-mode AD returns through the reference's rand(rng, fx, S)
+ * (test/finite_gp_projection.jl:105-127), for reparameterised Monte Carlo objectives and losses built on prior samples.
+ * With out = m + L Z, C = K + Sigma_y = L L', Obar the cotangent of out (N x S column-major, like Z) and V = L^-1:
+ *   z_bar = L' Obar                                   (N x S column-major, the cotangent of the normals Z)
+ *   mbar_i = sum_s Obar_is;  d/d ConstMean c = sum_i mbar_i
+ *   2 Cbar = V' Q V,  Q symmetric with the lower triangle (diagonal included) of z_bar Z'    (Murray 2016, symmetric form:
+ *            Lbar = tril(Obar Z'), and the lower triangle of L' Lbar is that of z_bar Z')
+ * and with W = 2 Cbar, exactly the reductions of agp_post_logpdf_grad_x with alpha = 0 and C^-1 replaced by -V'QV:
+ *   d/d theta = 1/2 sum_ij W_ij dK_ij/dtheta,  d/d sigma^2 = 1/2 tr W,  d/d sigma_i^2 = 1/2 W_ii,
+ *   x_grad[i, d] = sum_j W_ij d1k(x_i, x_j)_d.
+ * grad_out (double): the layout of agp_post_logpdf_grad -- 5 + D for a single kernel, agp_post_grad_len's composite layout
+ * for AGP_COMPOSITE; [3] is d/d sigma^2 of a scalar noise, [4] d/d ConstMean c.
+ * noise_diag_out / mean_diag_out: N values of `dtype` (d/d sigma_i^2, d/d m_i); x_grad_out: N x D values of `dtype` in
+ * `layout`, as agp_post_logpdf_grad_x's; z_bar_out: N x S values of `dtype`.  Under AGP_MEM_DEVICE, X, Z, out_bar and these
+ * four are DEVICE pointers.  Every output may be NULL, and its work is skipped (z_bar is formed whatever is requested; V,
+ * Q and the reductions only when grad_out, noise_diag_out or x_grad_out is requested).  A vector (CustomMean) mean and
+ * per-point noise are constants of X: the caller chains through mean_diag_out and noise_diag_out.
+ * Cost: the factor-only fit, then ~4 N^3 flop on the tile GEMM and the forward substitution (the substitution on the
+ * identity N^3, Q V 2 N^3, the lower half of V' (Q V) N^3), ~2x the logpdf gradient's.  Memory: the factor plus three
+ * N x N fp64 buffers whatever the dtype: (N + 128) N 8 + 3 N^2 8 bytes, plus O(N) terms (the int8-slice workspace of
+ * the substitution, ~7 kB per row) -- an estimate, ~65 GB at N = 45 000; the largest N that fits has not been measured.
+ * For AGP_F32 the pullback is formed in fp64 on the problem converted to fp64 and its outputs rounded to fp32: V'QV
+ * carries terms of the order of cond(C) that cancel.  mean_diag_out and grad_out[4] are summed in a fixed order; the
+ * other outputs are those of the reductions of agp_post_logpdf_grad_x (noise_diag_out and x_grad_out in a fixed order:
+ * two calls give the same bits).  Errors: a bad layout, S < 0, or a NULL X, or NULL Z / out_bar with S > 0:
+ * AGP_ERR_INVALID; a distributed context: AGP_ERR_UNSUPPORTED; C not positive definite: AGP_ERR_NOT_POSDEF with
+ * agp_last_info, as agp_rand; a failed device allocation: AGP_ERR_CUDA. */
+int32_t agp_rand_grad(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise,
+                      int32_t layout, const void* X, int64_t N, int32_t D, const void* Z, int32_t S,
+                      const void* out_bar, double* grad_out, void* noise_diag_out, void* mean_diag_out,
+                      void* x_grad_out, void* z_bar_out);
 
 /* ---- VFE (Titsias) -------------------------------------------------------------------------
  * approx_log_evidence(::VFE)/elbo src/sparse_approximations.jl:248-254 with

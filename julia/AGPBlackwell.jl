@@ -544,6 +544,69 @@ function CRC.rrule(::typeof(logpdf), fx::DevFiniteGP{T}, y::AbstractVector{<:Rea
     return lp, logpdf_pullback
 end
 
+# ---- reverse-mode rule for rand(rng, fx, S) (test/finite_gp_projection.jl:105-127) -----------------------------------
+# The forward pass draws Z exactly as the primal method above and calls agp_rand; the pullback sends the cotangent of the
+# samples through ONE agp_rand_grad call at the same Z (the factor is formed again there).  The tangents reuse the logpdf
+# rule's helpers; the rng gets NoTangent.  Unclaimed priors get no rule, so AD differentiates the stock method.
+# A CustomMean is a closure of x (and of whatever it captures) that the engine only sees evaluated: for such a prior the
+# rule differentiates `mean_split_rand` instead -- the closure's values plus a sample of the zero-mean prior, the same
+# numbers as the primal method (which adds the same T-rounded mean vector to the same L Z) -- so AD takes the closure's
+# own derivative with respect to x and its parameters, and only the zero-mean sample goes through agp_rand_grad.
+function composite_grad_len(k, D)   # the slots composite_grads reads, in agp_post_logpdf_grad's composite layout
+    n = 5
+    for (_, fs) in walk(k)
+        n += 1
+        for (leaf, _, tr) in fs
+            kind = transform_of(tr, D)[1]
+            n += kind == 1 ? 1 : (kind == 2 ? D : 0)
+            n += leaf isa Union{RationalQuadraticKernel,LinearKernel,ConstantKernel} ? 1 : 0
+            n += leaf isa PeriodicKernel ? D : 0
+        end
+    end
+    return n
+end
+
+mean_split_rand(rng, fx::DevFiniteGP{T}, S) where {T} =
+    T.(AbstractGPs.mean_vector(fx.f.mean, fx.x)) .+ Random.rand(rng, FiniteGP(GP(AbstractGPs.ZeroMean(), fx.f.kernel), fx.x, fx.Σy), S)
+
+function CRC.rrule(config::CRC.RuleConfig{>:CRC.HasReverseMode}, ::typeof(Random.rand), rng::Random.AbstractRNG,
+                   fx::DevFiniteGP{T}, S::Int) where {T}
+    claimed(fx.f) || return nothing
+    fx.f.mean isa AbstractGPs.CustomMean && return CRC.rrule_via_ad(config, mean_split_rand, rng, fx, S)
+    c = ctx(); X, layout, D = points(fx.x); N = length(fx); Z = randn(rng, T, N, S); out = similar(Z)
+    ks, k1 = kernel_spec(fx.f.kernel, T, D); ms, k2 = mean_spec(fx.f.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
+    lock(c.lock) do
+        GC.@preserve X k1 k2 k3 check(c, ccall((:agp_rand, libagp), Int32,
+            (Ptr{Cvoid}, Int32, Ref{AgpKernel}, Ref{AgpMean}, Ref{AgpNoise}, Int32, Ptr{Cvoid}, Int64, Int32, Ptr{Cvoid}, Int32, Ptr{Cvoid}),
+            c.h, agp_dtype(T), ks, ms, ns, layout, X, N, D, Z, S, out))
+    end
+    composite = !supported(fx.f)
+    function rand_pullback(Δ)
+        Δ = CRC.unthunk(Δ)
+        Δ isa CRC.AbstractZero && return CRC.NoTangent(), CRC.NoTangent(), CRC.ZeroTangent(), CRC.NoTangent()
+        Ō = convert(Matrix{T}, Δ)
+        g = Vector{Float64}(undef, composite ? composite_grad_len(fx.f.kernel, D) : 5 + D)
+        nd = Vector{T}(undef, N); xg = similar(X, T)
+        lock(c.lock) do
+            GC.@preserve X Ō g nd xg k1 k2 k3 check(c, ccall((:agp_rand_grad, libagp), Int32,
+                (Ptr{Cvoid}, Int32, Ref{AgpKernel}, Ref{AgpMean}, Ref{AgpNoise}, Int32, Ptr{Cvoid}, Int64, Int32, Ptr{Cvoid}, Int32,
+                 Ptr{Cvoid}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                c.h, agp_dtype(T), ks, ms, ns, layout, X, N, D, Z, S, Ō, g, nd, C_NULL, xg, C_NULL))
+        end
+        gs = (variance=g[1], scale=g[2], linear_c=g[3], noise=g[4], mean_c=g[5], ard=g[6:end], noise_diag=nd)
+        if composite
+            kt = ctangent(fx.f.kernel, Int[], composite_grads(fx.f.kernel, D, g), 1.0)
+        else
+            _, var, _, w = flat(fx.f.kernel)
+            kt = kernel_tangent(fx.f.kernel, gs, var, w === nothing ? 1.0 : w)
+        end
+        f̄ = CRC.Tangent{typeof(fx.f)}(; mean=mean_tangent(fx.f.mean, gs), kernel=kt)
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, xg), Σy=noise_tangent(fx.Σy, gs))
+        return CRC.NoTangent(), CRC.NoTangent(), f̄x, CRC.NoTangent()
+    end
+    return out, rand_pullback
+end
+
 # ---- reverse-mode rules for the VFE objectives: elbo(VFE(fz), fx, y) and approx_log_evidence(VFE | DTC, fx, y) ---------
 # (src/sparse_approximations.jl:248-254, :282-286).  One agp_vfe_elbo_grad_x call returns the value, the kernel / noise /
 # mean gradients in agp_post_logpdf_grad's layout (mapped back by the logpdf rule's helpers), the per-point noise and mean
