@@ -948,6 +948,71 @@ def logpdf_grad(fx: FiniteGP, y, inputs=False):
     return lp, out
 
 
+def loglikelihood_grad(fx: FiniteGP, Y, lp_bar=None, inputs=False):
+    """(logpdf vector, gradient dict) of sum_s lp_bar[s] * logpdf(fx, Y[:, s]) for a matrix Y (N x S, or a vector as one
+    column) over a prior GP -- what Zygote returns through the reference's logpdf(fx, Y::AbstractMatrix) and
+    loglikelihood(fx, Y) (test/finite_gp_projection.jl:165-178).  lp_bar=None is all ones: the gradient of
+    loglikelihood(fx, Y).  One fit and one agp_post_logpdf_grad_cols call whatever S is (one factorisation, one C^-1).
+    The dict has the keys of logpdf_grad ("kernel" for a composite, else "variance", "scale" | "ard", "linear_c"; "noise"
+    scalar or per-point; "mean_c" | "mean_v") and "Y", the cotangent of Y, shaped like Y.  inputs=True also returns
+    out["x"], the gradient with respect to the input points, shaped like the container fx was built from (RowVecs: N x D,
+    ColVecs: D x N, a vector: length N).  A CustomMean is treated as a constant of x: the caller chains through
+    out["mean_v"]."""
+    if not isinstance(fx.f, GP):
+        raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "the gradient of logpdf over a matrix Y is implemented for a FiniteGP over "
+                       "a prior GP, not over %s" % type(fx.f).__name__)
+    Yin = np.asarray(Y)
+    dt = fx.dtype
+    pts = fx.x.astype(dt)
+    N, D = pts.n, pts.D
+    Yf = np.asfortranarray(Yin.reshape(-1, 1) if Yin.ndim == 1 else Yin, dtype=dt)
+    if Yf.shape[0] != N:
+        raise DimensionMismatch("length(fx) = %d but Y has %d rows" % (N, Yf.shape[0]))
+    S = Yf.shape[1]
+    w = None if lp_bar is None else np.ascontiguousarray(lp_bar, dtype=np.float64).ravel()  # None: all ones
+    if w is not None and w.shape[0] != S:
+        raise DimensionMismatch("lp_bar has %d entries, Y has %d columns" % (w.shape[0], S))
+    lp, post = _fit(fx, Yf, True, False)
+    eng = engine()
+    f = fx.f
+    k = f.kernel
+    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
+    flat = _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D) if composite else None
+    g = np.zeros(flat.grad_len() if composite else 5 + D, dtype=np.float64)
+    per_point = np.ndim(fx.s2) != 0
+    nd = np.empty(N, dtype=dt) if per_point else None
+    md = np.empty(N, dtype=dt) if isinstance(f.mean, CustomMean) else None
+    yb = np.empty((N, S), dtype=dt, order="F")
+    # the points go in point-major, so x comes back point-major: D x N column-major, i.e. N x D row-major
+    xg = {"col": lambda: np.empty((D, N), dtype=dt, order="F"), "vec": lambda: np.empty(N, dtype=dt),
+          "row": lambda: np.empty((N, D), dtype=dt)}[fx.x_kind]() if inputs else None
+    keep = []
+    ms = _mean_struct(f.mean.spec(pts, dt), keep)
+    eng.check(eng.L.agp_post_logpdf_grad_cols(post.data.C.h, C.byref(ms), cabi.ptr(Yf), S,
+                                              None if w is None else w.ctypes.data_as(C.POINTER(C.c_double)),
+                                              g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), cabi.ptr(md),
+                                              cabi.AGP_POINT_MAJOR, cabi.ptr(xg), cabi.ptr(yb)))
+    if composite:
+        res = {"kernel": flat.params_grad(g)}
+    else:
+        res = {"variance": g[0]}
+        if isinstance(k.transform, ScaleTransform):
+            res["scale"] = g[1]
+        elif isinstance(k.transform, ARDTransform):
+            res["ard"] = g[5:5 + D].copy()
+        if k.family == LINEAR:
+            res["linear_c"] = g[2]
+    res["noise"] = nd.astype(np.float64) if per_point else g[3]
+    if isinstance(f.mean, ConstMean):
+        res["mean_c"] = g[4]
+    elif isinstance(f.mean, CustomMean):
+        res["mean_v"] = md.astype(np.float64)
+    res["Y"] = yb[:, 0].copy() if Yin.ndim == 1 else yb
+    if inputs:
+        res["x"] = xg
+    return np.atleast_1d(lp), res
+
+
 def _post_call(p: PosteriorGP, pts: _Points, s2, want_var=True, want_cov=False):
     eng = engine()
     dt = p.data.C.dtype

@@ -1294,33 +1294,154 @@ int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, dou
 }
 
 
+// what every logpdf gradient of a handle checks first: the input layout, the factor gathered whole, a handle straight
+// from agp_fit
 template <typename T>
-int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, int layout, void* x_grad_out) {
+int logpdf_grad_prelude(agp_post* p, int layout) {
   agp_ctx* ctx = p->ctx;
   if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
   { int rrc = post_replicate<T>(p); if (rrc) return rrc; }
-  cudaStream_t s = ctx->stream;
   CK(cudaSetDevice(ctx->device));
   if (p->valid || p->segs.size() > 1) { ctx->err = "gradient of an extended (sequentially conditioned) posterior is unsupported"; return AGP_ERR_UNSUPPORTED; }
+  return AGP_OK;
+}
+
+// V = L^-1 by the blocked forward substitution on the identity and, with want_cinv, C^-1 = V'V into its lower tiles: two
+// n_pad x n_pad buffers of the call's scratch (Cinv stays null without want_cinv)
+template <typename T>
+int inverse_factor(agp_post* p, Scratch& sc, bool want_cinv, T** V_out, T** Cinv_out) {
+  agp_ctx* ctx = p->ctx;
+  cudaStream_t s = ctx->stream;
   const int64_t n_pad = p->n_pad;
-  if (!grad_out && !noise_diag_out && !x_grad_out) return AGP_OK;
-  Scratch sc(ctx);
   void* tmp = nullptr;
   CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
   T* V = (T*)tmp;
-  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
-  T* Cinv = (T*)tmp;
+  T* Cinv = nullptr;
+  if (want_cinv) { CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T))); Cinv = (T*)tmp; }
   CK(cudaMemsetAsync(V, 0, (size_t)n_pad * n_pad * sizeof(T), s));
   launch_add_diag<T>(V, n_pad, n_pad, 1.0, s);
   forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, V, n_pad, n_pad);
-  {
+  if (want_cinv) {
     GemmArgs g{};  // C^-1 = V'V, lower tiles
     g.A = V; g.lda = n_pad; g.a_kmajor = 1;
     g.B = V; g.ldb = n_pad; g.b_kmajor = 1;
     g.C = Cinv; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = 1;
     launch_gemm<T>(g, s);
   }
+  *V_out = V; *Cinv_out = Cinv;
+  return AGP_OK;
+}
+
+template <typename T>
+int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, int layout, void* x_grad_out) {
+  int rc = logpdf_grad_prelude<T>(p, layout);
+  if (rc) return rc;
+  if (!grad_out && !noise_diag_out && !x_grad_out) return AGP_OK;
+  Scratch sc(p->ctx);
+  T *V = nullptr, *Cinv = nullptr;
+  rc = inverse_factor<T>(p, sc, true, &V, &Cinv);
+  if (rc) return rc;
   return grad_reductions<T>(p, sc, Cinv, (const T*)p->alpha, grad_out, noise_diag_out, layout, x_grad_out);
+}
+
+// ---- pullback of sum_s w_s logpdf(fx, Y[:, s]) on a handle from agp_fit (agp.h agp_post_logpdf_grad_cols).  With
+// delta_s = Y[:, s] - m, A = C^-1 [delta_1 .. delta_S] and w = lp_bar:
+//   -W = (sum_s w_s) C^-1 - A diag(w) A'   into the lower tiles of the C^-1 buffer,  mbar = A w,  Ybar = -A diag(w)
+// and then the reductions of agp_post_logpdf_grad_x with alpha = 0 and C^-1 replaced by -W.  The columns go through in
+// chunks of up to 1024 (fit_many_impl's): Delta_c = Y_c - m, B_c = L^-1 Delta_c, A_c = V' B_c on the tile GEMM (V = L^-1,
+// as C^-1 = V'V is formed: the same accuracy class), Ybar_c = A_c diag(-w_c), -W += Ybar_c A_c' (a rank-nc lower-only
+// GEMM), mbar += A_c w_c.  Two n_pad x n_pad and two n_pad x 1024 buffers of T whatever S is.
+template <typename T>
+int post_logpdf_grad_cols_impl(agp_post* p, const agp_mean* mean, const void* Y, int S, const double* lp_bar,
+                               double* grad_out, void* noise_diag_out, void* mean_diag_out, int layout, void* x_grad_out,
+                               void* y_bar_out) {
+  agp_ctx* ctx = p->ctx;
+  if (S < 1) { ctx->err = "S must be >= 1"; return AGP_ERR_INVALID; }
+  if (!Y) { ctx->err = "Y is NULL"; return AGP_ERR_INVALID; }
+  if (mean && mean->kind == 2 && !mean->v) { ctx->err = "mean vector is NULL"; return AGP_ERR_INVALID; }
+  int rc = logpdf_grad_prelude<T>(p, layout);
+  if (rc) return rc;
+  const bool want_w = grad_out || noise_diag_out || x_grad_out;
+  const bool want_mbar = grad_out || mean_diag_out;
+  if (!want_w && !want_mbar && !y_bar_out) return AGP_OK;
+  const agp_mean handle_mean{p->mean_kind, p->mean_c, nullptr};
+  if (!mean) mean = &handle_mean;
+  cudaStream_t s = ctx->stream;
+  const int64_t N = p->n, n_pad = p->n_pad;
+  const int64_t chunk = 1024, cmax = round_up(S < chunk ? S : chunk, TILE);
+  Scratch sc(ctx);
+  T *V = nullptr, *Cinv = nullptr;  // Cinv becomes -W
+  rc = inverse_factor<T>(p, sc, want_w, &V, &Cinv);
+  if (rc) return rc;
+  void* tmp = nullptr;
+  CK(sc.alloc(&tmp, (size_t)n_pad * cmax * sizeof(T) * 2));
+  T* B = (T*)tmp;  // Delta_c, L^-1 Delta_c, then Ybar_c
+  T* A = B + n_pad * cmax;
+  std::vector<double> w((size_t)S, 1.0);
+  if (lp_bar) w.assign(lp_bar, lp_bar + S);
+  double wsum = 0.0;
+  for (double v : w) wsum += v;
+  std::vector<T> hw((size_t)2 * S);  // w, then -w
+  for (int j = 0; j < S; ++j) { hw[(size_t)j] = (T)w[(size_t)j]; hw[(size_t)S + j] = (T)-w[(size_t)j]; }
+  T* wd = nullptr;
+  rc = upload<T>(ctx, sc, hw.data(), hw.size(), true, &wd);
+  if (rc) return rc;
+  T *mbar = nullptr, *mean_d = nullptr;
+  if (want_mbar) { CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T))); mbar = (T*)tmp; CK(cudaMemsetAsync(mbar, 0, (size_t)n_pad * sizeof(T), s)); }
+  if (mean->kind == 2) { rc = upload<T>(ctx, sc, mean->v, N, true, &mean_d); if (rc) return rc; }
+  if (want_w && wsum != 1.0) launch_scale<T>(Cinv, n_pad * n_pad, wsum, s);
+  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  for (int64_t c0 = 0; c0 < S; c0 += chunk) {
+    const int64_t nc = (S - c0 < chunk) ? (S - c0) : chunk, nc_pad = round_up(nc, TILE);
+    Scratch scc(ctx);
+    T* Yd = nullptr;
+    rc = upload<T>(ctx, scc, (const T*)Y + (size_t)c0 * N, (size_t)N * nc, false, &Yd);
+    if (rc) return rc;
+    launch_sub_mean_cols<T>(Yd, N, N, nc, mean->kind, mean->c, mean_d, B, n_pad, n_pad, nc_pad, s);
+    forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, B, n_pad, nc_pad);
+    {
+      GemmArgs g{};  // A_c = V' B_c
+      g.A = V; g.lda = n_pad; g.a_kmajor = 1;
+      g.B = B; g.ldb = n_pad; g.b_kmajor = 1;
+      g.C = A; g.ldc = n_pad; g.M = n_pad; g.N = nc_pad; g.K = n_pad;
+      launch_gemm<T>(g, s);
+    }
+    if (want_mbar) launch_gemv_n_acc<T>(A, n_pad, N, nc, wd + c0, mbar, s);
+    CK(cudaMemcpyAsync(B, A, (size_t)n_pad * nc_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    launch_scale_cols<T>(B, n_pad, n_pad, nc, wd + S + c0, s);  // Ybar_c = A_c diag(-w_c)
+    if (want_w) {
+      GemmArgs g{};  // -W += Ybar_c A_c', lower tiles
+      g.A = B; g.lda = n_pad; g.a_kmajor = 0;
+      g.B = A; g.ldb = n_pad; g.b_kmajor = 0;
+      g.C = Cinv; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = nc_pad; g.beta_one = 1; g.lower_only = 1;
+      launch_gemm<T>(g, s);
+    }
+    if (y_bar_out)
+      CK(cudaMemcpy2DAsync((T*)y_bar_out + (size_t)c0 * N, (size_t)N * sizeof(T), B, (size_t)n_pad * sizeof(T), (size_t)N * sizeof(T),
+                           (size_t)nc, kout, s));
+  }
+  if (want_w) {
+    CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T)));
+    T* zero_alpha = (T*)tmp;
+    CK(cudaMemsetAsync(zero_alpha, 0, (size_t)n_pad * sizeof(T), s));
+    rc = grad_reductions<T>(p, sc, Cinv, zero_alpha, grad_out, noise_diag_out, layout, x_grad_out);
+    if (rc) return rc;
+  }
+  if (want_mbar) {
+    rc = download<T>(ctx, mean_diag_out, mbar, (size_t)N, false);
+    if (rc) return rc;
+  }
+  if (grad_out) {  // d/d ConstMean c = sum_i mbar_i, in index order
+    std::vector<T> h((size_t)N);
+    CK(cudaMemcpyAsync(h.data(), mbar, (size_t)N * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    double c = 0.0;
+    for (int64_t i = 0; i < N; ++i) c += (double)h[(size_t)i];
+    grad_out[4] = c;
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return AGP_OK;
 }
 
 template <typename T>
@@ -2999,6 +3120,17 @@ int32_t agp_post_logpdf_grad_x(agp_post* p, double* grad_out, void* noise_diag_o
   if (!p) return AGP_ERR_INVALID;
   return DISPATCH(p->dtype, post_logpdf_grad_impl<float>(p, grad_out, noise_diag_out, layout, x_grad_out),
                   post_logpdf_grad_impl<double>(p, grad_out, noise_diag_out, layout, x_grad_out));
+}
+
+int32_t agp_post_logpdf_grad_cols(agp_post* p, const agp_mean* mean, const void* Y, int32_t S, const double* lp_bar,
+                                  double* grad_out, void* noise_diag_out, void* mean_diag_out, int32_t layout,
+                                  void* x_grad_out, void* y_bar_out) {
+  if (!p) return AGP_ERR_INVALID;
+  return DISPATCH(p->dtype,
+                  post_logpdf_grad_cols_impl<float>(p, mean, Y, S, lp_bar, grad_out, noise_diag_out, mean_diag_out, layout,
+                                                    x_grad_out, y_bar_out),
+                  post_logpdf_grad_cols_impl<double>(p, mean, Y, S, lp_bar, grad_out, noise_diag_out, mean_diag_out, layout,
+                                                     x_grad_out, y_bar_out));
 }
 
 int32_t agp_post_solve_lower(agp_post* p, const void* B, int64_t nrhs, void* V_out) {

@@ -131,6 +131,11 @@ template <typename T> void launch_cov_finish(T* C, int64_t ldc, const T* Kss, in
 template <typename T> void launch_fill(T* p, int64_t n, double v, cudaStream_t s);
 // out[i] = y[i] - mean_i
 template <typename T> void launch_sub_mean(const T* y, int64_t n, int mean_kind, double mean_c, const T* mean_v, T* out, cudaStream_t s);
+// out[i + j*ldo] = Y[i + j*ldy] - mean_i for i < n, j < nc; 0 elsewhere in the n_pad x nc_pad block
+template <typename T> void launch_sub_mean_cols(const T* Y, int64_t ldy, int64_t n, int64_t nc, int mean_kind, double mean_c,
+                                                const T* mean_v, T* out, int64_t ldo, int64_t n_pad, int64_t nc_pad, cudaStream_t s);
+// p[i] *= v for i < n
+template <typename T> void launch_scale(T* p, int64_t n, double v, cudaStream_t s);
 // y[m] += sum_n A[m + n*lda] * x[n]   (rows coalesced)
 template <typename T> void launch_gemv_n_acc(const T* A, int64_t lda, int64_t m, int64_t n, const T* x, T* y, cudaStream_t s);
 // out[j] += sign * sum_i V[i + j*ldv]^2

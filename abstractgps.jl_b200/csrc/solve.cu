@@ -445,6 +445,24 @@ __global__ void sub_mean_kernel(const T* __restrict__ y, int64_t n, int mean_kin
   T m = (mean_kind == 0) ? (T)0 : (mean_kind == 1 ? mean_c : mean_v[i]);
   out[i] = y[i] - m;
 }
+
+// one column block of Y - m, zero-padded to n_pad rows and gridDim.y columns (the multi-column logpdf gradient)
+template <typename T>
+__global__ void sub_mean_cols_kernel(const T* __restrict__ Y, int64_t ldy, int64_t n, int64_t nc, int mean_kind, T mean_c,
+                                     const T* __restrict__ mean_v, T* __restrict__ out, int64_t ldo, int64_t n_pad) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  const int64_t j = blockIdx.y;
+  if (i >= n_pad) return;
+  T v = (T)0;
+  if (i < n && j < nc) v = Y[i + j * ldy] - ((mean_kind == 0) ? (T)0 : (mean_kind == 1 ? mean_c : mean_v[i]));
+  out[i + j * ldo] = v;
+}
+
+template <typename T>
+__global__ void scale_kernel(T* __restrict__ p, int64_t n, T v) {
+  const int64_t i = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
+  if (i < n) p[i] *= v;
+}
 }  // namespace
 
 template <typename T>
@@ -590,6 +608,20 @@ void launch_sub_mean(const T* y, int64_t n, int mean_kind, double mean_c, const 
   sub_mean_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(y, n, mean_kind, (T)mean_c, mean_v, out);
   agp_count_launch();
 }
+template <typename T>
+void launch_sub_mean_cols(const T* Y, int64_t ldy, int64_t n, int64_t nc, int mean_kind, double mean_c, const T* mean_v, T* out,
+                          int64_t ldo, int64_t n_pad, int64_t nc_pad, cudaStream_t s) {
+  if (n_pad <= 0 || nc_pad <= 0) return;
+  dim3 grid((unsigned)((n_pad + 255) / 256), (unsigned)nc_pad);
+  sub_mean_cols_kernel<T><<<grid, 256, 0, s>>>(Y, ldy, n, nc, mean_kind, (T)mean_c, mean_v, out, ldo, n_pad);
+  agp_count_launch();
+}
+template <typename T>
+void launch_scale(T* p, int64_t n, double v, cudaStream_t s) {
+  if (n <= 0) return;
+  scale_kernel<T><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(p, n, (T)v);
+  agp_count_launch();
+}
 
 template <typename T>
 void launch_border_init_cols(T* A, int64_t lda, int64_t row_off, int64_t col0, int64_t ncols, int64_t n, const T* Y,
@@ -663,6 +695,12 @@ template void launch_bwd_diag<double>(const double*, const double*, double*, cud
 template void launch_bwd_update_local<double>(const double*, int64_t, int, const double*, double*, int, int, int, int, cudaStream_t);
 template void launch_sub_mean<float>(const float*, int64_t, int, double, const float*, float*, cudaStream_t);
 template void launch_sub_mean<double>(const double*, int64_t, int, double, const double*, double*, cudaStream_t);
+template void launch_sub_mean_cols<float>(const float*, int64_t, int64_t, int64_t, int, double, const float*, float*, int64_t,
+                                          int64_t, int64_t, cudaStream_t);
+template void launch_sub_mean_cols<double>(const double*, int64_t, int64_t, int64_t, int, double, const double*, double*, int64_t,
+                                           int64_t, int64_t, cudaStream_t);
+template void launch_scale<float>(float*, int64_t, double, cudaStream_t);
+template void launch_scale<double>(double*, int64_t, double, cudaStream_t);
 template void launch_gemv_n_acc<float>(const float*, int64_t, int64_t, int64_t, const float*, float*, cudaStream_t);
 template void launch_colsumsq_acc<float>(const float*, int64_t, int64_t, int64_t, double, float*, cudaStream_t);
 template void launch_zero_diag_upper<float>(float*, int64_t, int64_t, cudaStream_t);

@@ -212,6 +212,36 @@ int32_t agp_post_logpdf_grad(agp_post* p, double* grad_out, void* noise_diag_out
  * other than the two gives AGP_ERR_INVALID.  agp_post_logpdf_grad(p, g, nd) is agp_post_logpdf_grad_x(p, g, nd,
  * AGP_POINT_MAJOR, NULL). */
 int32_t agp_post_logpdf_grad_x(agp_post* p, double* grad_out, void* noise_diag_out, int32_t layout, void* x_grad_out);
+/* The gradient of sum_s w_s logpdf(fx, Y[:, s]) for a matrix Y (N x S column-major, any S >= 1) from the factor of the
+ * handle, with w = lp_bar the cotangent of the S-vector of logpdfs: what reverse-mode AD returns through the reference's
+ * logpdf(fx, Y::AbstractMatrix) and loglikelihood(fx, Y) (test/finite_gp_projection.jl:165-178; w = 1 for loglikelihood).
+ * With delta_s = Y[:, s] - m, alpha_s = C^-1 delta_s, A = [alpha_1 .. alpha_S] and
+ *   W = A diag(w) A' - (sum_s w_s) C^-1
+ * the outputs are the reductions of agp_post_logpdf_grad_x with this W in place of alpha alpha' - C^-1:
+ *   d/d theta = 1/2 sum_ij W_ij dK_ij/dtheta,  d/d sigma^2 = 1/2 tr W,  d/d sigma_i^2 = 1/2 W_ii,
+ *   x_grad[i, d] = sum_j W_ij d1k(x_i, x_j)_d,  mbar = A w (d/d m_i),  d/d ConstMean c = sum_i mbar_i,
+ *   y_bar = -A diag(w)  (N x S column-major, the cotangent of Y).
+ * The pullback is evaluated at this Y, which need not be the one the handle was fit with.  mean: the prior mean at the
+ * handle's points (host arrays); NULL means the handle's zero or constant mean.  The handle keeps no vector mean, so a
+ * CustomMean's values must be passed again.  lp_bar: S host doubles; NULL means all ones.
+ * grad_out (double): the layout of agp_post_logpdf_grad -- 5 + D for a single kernel, agp_post_grad_len(p) for a
+ * composite; [3] is 1/2 tr W, [4] sum_i mbar_i.  noise_diag_out, mean_diag_out (N values each) and y_bar_out (N x S) have
+ * the handle's dtype; x_grad_out is in `layout`, as agp_post_logpdf_grad_x's.  Under AGP_MEM_DEVICE, Y and these four are
+ * DEVICE pointers.  Every output may be NULL, and its work is skipped (C^-1, the rank-S updates and the reductions run
+ * only for grad_out, noise_diag_out or x_grad_out).
+ * Arithmetic: that of agp_post_logpdf_grad_x in the handle's dtype (V = L^-1, C^-1 and A in T, the sums in fp64), so at
+ * S = 1, w = 1 the two agree to the dtype's rounding.  A = V' (L^-1 Delta) is formed on the tile GEMM in column chunks of
+ * up to 1024.  Cost: the logpdf gradient's ~2 N^3 flop (V and C^-1 = V'V), plus ~N^2 S for the substitution of the
+ * columns, 2 N^2 S for A and N^2 S for the lower half of the rank-S update: ~4 N^2 S flop.  Memory: besides the handle,
+ * two N x N buffers of T (as agp_post_logpdf_grad_x), two N x min(S, 1024) chunk buffers and, for a host Y, the copy of
+ * one chunk of it; nothing else grows with S.
+ * Determinism: noise_diag_out, mean_diag_out, x_grad_out and y_bar_out are formed in a fixed order (two calls give the
+ * same bits), grad_out[4] too; the other entries of grad_out leave their CTAs through fp64 atomics and agree to rounding.
+ * Errors: S < 1, a NULL Y, a bad layout, or a vector mean with a NULL v: AGP_ERR_INVALID; an extended handle:
+ * AGP_ERR_UNSUPPORTED; a failed device allocation: AGP_ERR_CUDA. */
+int32_t agp_post_logpdf_grad_cols(agp_post* p, const agp_mean* mean, const void* Y, int32_t S, const double* lp_bar,
+                                  double* grad_out, void* noise_diag_out, void* mean_diag_out, int32_t layout,
+                                  void* x_grad_out, void* y_bar_out);
 /* number of doubles agp_post_logpdf_grad writes: 5 + D for a single kernel, the layout above for a composite */
 int64_t agp_post_grad_len(const agp_post* p);
 /* V = U' \ B (N x nrhs, column-major): backs Xt_invA_X / diag_Xt_invA_X / Xt_invA_Y /

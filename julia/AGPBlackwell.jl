@@ -544,6 +544,45 @@ function CRC.rrule(::typeof(logpdf), fx::DevFiniteGP{T}, y::AbstractVector{<:Rea
     return lp, logpdf_pullback
 end
 
+# ---- reverse-mode rule for logpdf(fx, Y) with a matrix Y (test/finite_gp_projection.jl:165-178) ------------------------
+# The forward pass is one fit that keeps the handle; the pullback receives the S-vector of cotangents Δ and makes ONE
+# agp_post_logpdf_grad_cols call with lp_bar = Δ, so one factorisation and one C^-1 serve every column.
+# loglikelihood(fx, Y) = sum(logpdf(fx, Y)) differentiates through this rule.  The tangents are mapped back by the helpers
+# of the rules above; Ȳ is the tangent of Y.  A CustomMean's values go to the call again (the handle keeps none), and the
+# closure is not differentiated, as in the vector rule.
+function CRC.rrule(::typeof(logpdf), fx::DevFiniteGP{T}, Y::AbstractMatrix{<:Real}) where {T}
+    claimed(fx.f) || return nothing                                       # no rule: AD differentiates the stock method
+    lp, post = fit(fx, Y)
+    c = ctx(); X, layout, D = points(fx.x); N = length(fx); S = size(Y, 2)
+    Ym = convert(Matrix{T}, Y)
+    ms, k2 = mean_spec(fx.f.mean, fx.x, T)
+    composite = !supported(fx.f)
+    function logpdf_matrix_pullback(Δ)
+        Δ = CRC.unthunk(Δ)
+        Δ isa CRC.AbstractZero && return CRC.NoTangent(), CRC.ZeroTangent(), CRC.ZeroTangent()
+        w = convert(Vector{Float64}, Δ)
+        glen = composite ? ccall((:agp_post_grad_len, libagp), Int64, (Ptr{Cvoid},), post.data.C.h) : 5 + D
+        g = Vector{Float64}(undef, glen); nd = Vector{T}(undef, N); xg = similar(X, T); Ȳ = Matrix{T}(undef, N, S)
+        lock(c.lock) do
+            GC.@preserve Ym w g nd xg Ȳ k2 check(c, ccall((:agp_post_logpdf_grad_cols, libagp), Int32,
+                (Ptr{Cvoid}, Ref{AgpMean}, Ptr{Cvoid}, Int32, Ptr{Float64}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Cvoid}, Int32,
+                 Ptr{Cvoid}, Ptr{Cvoid}),
+                post.data.C.h, ms, Ym, S, w, g, nd, C_NULL, layout, xg, Ȳ))
+        end
+        gs = (variance=g[1], scale=g[2], linear_c=g[3], noise=g[4], mean_c=g[5], ard=g[6:end], noise_diag=nd)
+        if composite
+            kt = ctangent(fx.f.kernel, Int[], composite_grads(fx.f.kernel, D, g), 1.0)
+        else
+            _, var, _, wt = flat(fx.f.kernel)
+            kt = kernel_tangent(fx.f.kernel, gs, var, wt === nothing ? 1.0 : wt)
+        end
+        f̄ = CRC.Tangent{typeof(fx.f)}(; mean=mean_tangent(fx.f.mean, gs), kernel=kt)
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, xg), Σy=noise_tangent(fx.Σy, gs))
+        return CRC.NoTangent(), f̄x, Ȳ
+    end
+    return lp, logpdf_matrix_pullback
+end
+
 # ---- reverse-mode rule for rand(rng, fx, S) (test/finite_gp_projection.jl:105-127) -----------------------------------
 # The forward pass draws Z exactly as the primal method above and calls agp_rand; the pullback sends the cotangent of the
 # samples through ONE agp_rand_grad call at the same Z (the factor is formed again there).  The tangents reuse the logpdf
