@@ -80,6 +80,8 @@ SIGNATURES = {
     "agp_post_logpdf_grad_x": (C.c_int32, [_P, C.POINTER(C.c_double), _P, C.c_int32, _P]),
     "agp_post_logpdf_grad_cols": (C.c_int32, [_P, _M, _P, C.c_int32, C.POINTER(C.c_double), C.POINTER(C.c_double), _P, _P,
                                               C.c_int32, _P, _P]),
+    "agp_post_pred_logpdf_grad": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _M, _N, _P, C.c_int32, C.POINTER(C.c_double), _P,
+                                              C.POINTER(C.c_double), _P, _P, _P, _P, _P, _P, _P, _P]),
     "agp_post_grad_len": (C.c_int64, [_P]),
     "agp_post_solve_lower": (C.c_int32, [_P, _P, C.c_int64, _P]),
     "agp_post_factor_export": (C.c_int32, [_P, _P]),

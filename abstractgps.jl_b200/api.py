@@ -818,7 +818,9 @@ def _fit(fx: FiniteGP, Y, want_post: bool, want_alpha: bool):
         return lpv, None
     delta = Yf[:, 0] - f.mean.vector(pts, dt)
     data = DeviceData(alpha=alpha, C=DeviceCholesky(eng, post, dt), x=fx.x, delta=delta)
-    return lpv, PosteriorGP(f, data)
+    p = PosteriorGP(f, data)
+    p.fx = fx  # the FiniteGP it was conditioned on: its noise and input container shape the posterior's gradients
+    return lpv, p
 
 
 def logpdf(fx: FiniteGP, y):
@@ -1011,6 +1013,79 @@ def loglikelihood_grad(fx: FiniteGP, Y, lp_bar=None, inputs=False):
     if inputs:
         res["x"] = xg
     return np.atleast_1d(lp), res
+
+
+def posterior_logpdf_grad(fx: FiniteGP, Y, lp_bar=None, inputs=False):
+    """(logpdf, gradient dict) of sum_s lp_bar[s] * logpdf(fx, Y[:, s]) for fx = p(x*, s2*) over an exact posterior
+    p = posterior(fx0, y): the held-out log-likelihood logpdf(posterior(fx0, y)(x*, s2*), y*) differentiated with respect
+    to both the training and the test side, in one agp_post_pred_logpdf_grad call on p's handle.  Y is M x S (or a vector
+    as one column); lp_bar=None is all ones.  The dict has the kernel keys of logpdf_grad ("kernel" for a composite, else
+    "variance", "scale" | "ard", "linear_c"), the training side "noise" (scalar or per-point, as fx0's noise), "mean_c"
+    (ConstMean) or "mean_v" (CustomMean, at x) and "y" (the cotangent of y); the test side "noise_s" (scalar or per-point,
+    as fx's noise), "mean_s_v" (CustomMean, at x*) and "Y" (shaped like Y).  A ConstMean's "mean_c" counts both sides.
+    inputs=True also returns "x" and "xs", the gradients with respect to the training and the test inputs, shaped like the
+    containers they came in (RowVecs: N x D, ColVecs: D x N, a vector: length N).  A CustomMean is treated as a constant
+    of the inputs.  Only a posterior straight from posterior(fx0, y) is supported (not a sequentially conditioned one)."""
+    p = fx.f
+    if not isinstance(p, PosteriorGP) or getattr(p, "fx", None) is None:
+        raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "the gradient of the held-out logpdf needs a FiniteGP over posterior(fx, y), "
+                       "not over %s" % type(p).__name__)
+    eng = engine()
+    p, dt, pts, ms, ns, keep = _post_args(fx)
+    fx0 = p.fx
+    N, M, D = p.data.x.n, pts.n, pts.D
+    Yin = np.asarray(Y)
+    Yf = np.asfortranarray(Yin.reshape(-1, 1) if Yin.ndim == 1 else Yin, dtype=dt)
+    if Yf.shape[0] != M:
+        raise DimensionMismatch("length(fx) = %d but Y has %d rows" % (M, Yf.shape[0]))
+    S = Yf.shape[1]
+    w = None if lp_bar is None else np.ascontiguousarray(lp_bar, dtype=np.float64).ravel()  # None: all ones
+    if w is not None and w.shape[0] != S:
+        raise DimensionMismatch("lp_bar has %d entries, Y has %d columns" % (w.shape[0], S))
+    f = p.prior
+    k = f.kernel
+    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
+    g = np.zeros(int(eng.L.agp_post_grad_len(p.data.C.h)) if composite else 5 + D, dtype=np.float64)
+    lp = np.empty(S, dtype=dt)
+    nd = np.empty(N, dtype=dt) if np.ndim(fx0.s2) != 0 else None
+    md = np.empty(N, dtype=dt) if isinstance(f.mean, CustomMean) else None
+    yb = np.empty(N, dtype=dt)
+    nsd = np.empty(M, dtype=dt)
+    msd = np.empty(M, dtype=dt) if isinstance(f.mean, CustomMean) else None
+    ysb = np.empty((M, S), dtype=dt, order="F")
+    # the points go in point-major, so the input gradients come back point-major: D x n column-major, n x D row-major
+    shape = lambda kind, n: {"col": lambda: np.empty((D, n), dtype=dt, order="F"), "vec": lambda: np.empty(n, dtype=dt),
+                             "row": lambda: np.empty((n, D), dtype=dt)}[kind]()
+    xg = shape(fx0.x_kind, N) if inputs else None
+    xsg = shape(fx.x_kind, M) if inputs else None
+    dbl = lambda a: None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
+    eng.check(eng.L.agp_post_pred_logpdf_grad(p.data.C.h, cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), M, C.byref(ms), C.byref(ns),
+                                              cabi.ptr(Yf), S, dbl(w), cabi.ptr(lp), dbl(g), cabi.ptr(nd), cabi.ptr(md),
+                                              cabi.ptr(yb), cabi.ptr(xg), cabi.ptr(nsd), cabi.ptr(msd), cabi.ptr(ysb),
+                                              cabi.ptr(xsg)))
+    if composite:
+        res = {"kernel": _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D).params_grad(g)}
+    else:
+        res = {"variance": g[0]}
+        if isinstance(k.transform, ScaleTransform):
+            res["scale"] = g[1]
+        elif isinstance(k.transform, ARDTransform):
+            res["ard"] = g[5:5 + D].copy()
+        if k.family == LINEAR:
+            res["linear_c"] = g[2]
+    res["noise"] = nd.astype(np.float64) if nd is not None else g[3]
+    if isinstance(f.mean, ConstMean):
+        res["mean_c"] = g[4]
+    elif isinstance(f.mean, CustomMean):
+        res["mean_v"] = md.astype(np.float64)
+    res["y"] = yb
+    res["noise_s"] = nsd.astype(np.float64) if np.ndim(fx.s2) != 0 else float(np.sum(nsd, dtype=np.float64))
+    if msd is not None:
+        res["mean_s_v"] = msd.astype(np.float64)
+    res["Y"] = ysb[:, 0].copy() if Yin.ndim == 1 else ysb
+    if inputs:
+        res["x"], res["xs"] = xg, xsg
+    return (lp[0] if Yin.ndim == 1 else lp), res
 
 
 def _post_call(p: PosteriorGP, pts: _Points, s2, want_var=True, want_cov=False):

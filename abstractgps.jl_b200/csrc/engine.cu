@@ -1215,12 +1215,13 @@ static CompositeDesc single_kernel_desc(int family, double variance, double line
 //   grad_out = the agp_post_logpdf_grad layout of 1/2 sum_ij W_ij dC_ij/dtheta ([3] = 1/2 tr W, [4] = sum alpha),
 //   noise_diag_out = 1/2 W_ii,  x_grad_out = sum_j W_ij d1k(x_i, x_j)  (agp_post_logpdf_grad_x).
 // Any output may be NULL.  agp_post_logpdf_grad_x runs it with C^-1; agp_rand_grad with alpha = 0 and Cinv = -V'QV.
+// grad_reductions_on runs the same reductions with the handle's kernel over another point set X (n points, n_pad rows,
+// transformed like the handle's) and a W of leading dimension ldc: agp_post_pred_logpdf_grad's stacked [x; x*].
 template <typename T>
-int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, double* grad_out, void* noise_diag_out, int layout,
-                    void* x_grad_out) {
+int grad_reductions_on(agp_post* p, Scratch& sc, const T* X, int64_t n, int64_t n_pad, const T* Cinv, int64_t ldc,
+                       const T* alpha, double* grad_out, void* noise_diag_out, int layout, void* x_grad_out) {
   agp_ctx* ctx = p->ctx;
   cudaStream_t s = ctx->stream;
-  const int64_t n = p->n, n_pad = p->n_pad;
   const int D = p->D;
   const bool want_theta = grad_out || noise_diag_out;  // the hyper-parameter reduction also yields noise_diag
   void* tmp = nullptr;
@@ -1233,10 +1234,9 @@ int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, dou
   const int want_ard = (p->k.transform == AGP_T_ARD) ? 1 : 0;
   if (want_theta) {
     if (p->comp)
-      launch_composite_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, alpha, p->comp->desc, sums, noise_d, s);
+      launch_composite_grad_reduce<T>(X, D, n, n_pad, Cinv, ldc, alpha, p->comp->desc, sums, noise_d, s);
     else
-      launch_grad_reduce<T>((const T*)p->Xt, D, n, n_pad, Cinv, n_pad, alpha, p->k.family, p->k.linear_c, want_ard,
-                            sums, noise_d, s);
+      launch_grad_reduce<T>(X, D, n, n_pad, Cinv, ldc, alpha, p->k.family, p->k.linear_c, want_ard, sums, noise_d, s);
   }
   if (x_grad_out) {  // sum_j W_ij d1k(x_i, x_j) from the same W (grad_x.cu)
     const CompositeDesc one = single_kernel_desc(p->k.family, p->k.variance, p->k.linear_c);
@@ -1253,7 +1253,7 @@ int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, dou
     double* part = (double*)tmp;
     CK(sc.alloc(&tmp, (size_t)n * D * sizeof(T)));
     T* xg = (T*)tmp;
-    launch_grad_x<T>((const T*)p->Xt, D, n, Cinv, n_pad, alpha, *cd, mult, ard, layout, part, xg, s);
+    launch_grad_x<T>(X, D, n, Cinv, ldc, alpha, *cd, mult, ard, layout, part, xg, s);
     int rc = download<T>(ctx, x_grad_out, xg, (size_t)n * D, false); if (rc) return rc;
   }
   if (!want_theta) {
@@ -1291,6 +1291,13 @@ int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, dou
   for (int d = 0; d < D; ++d)
     grad_out[5 + d] = want_ard ? (linear ? var : 0.5 * var) * h[(size_t)5 + d] / (double)ard_h[(size_t)d] : 0.0;
   return AGP_OK;
+}
+
+template <typename T>
+int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, double* grad_out, void* noise_diag_out, int layout,
+                    void* x_grad_out) {
+  return grad_reductions_on<T>(p, sc, (const T*)p->Xt, p->n, p->n_pad, Cinv, p->n_pad, alpha, grad_out, noise_diag_out,
+                               layout, x_grad_out);
 }
 
 
@@ -1438,6 +1445,292 @@ int post_logpdf_grad_cols_impl(agp_post* p, const agp_mean* mean, const void* Y,
     double c = 0.0;
     for (int64_t i = 0; i < N; ++i) c += (double)h[(size_t)i];
     grad_out[4] = c;
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return AGP_OK;
+}
+
+// ---- pullback of F = sum_s w_s logpdf(posterior(fx, y)(x*, Sigma*), Y*[:, s]) on a handle from agp_fit (agp.h
+// agp_post_pred_logpdf_grad).  With C = L L', alpha = C^-1 delta, A = L^-1 K_xs, P = C^-1 K_xs = V'A (V = L^-1),
+// mu* = m* + K_sx alpha, Sigma = K_ss - A'A + Sigma* = L* L*' and E = Y* - mu* 1':
+//   -2 Sigmabar = (sum w) Sigma^-1 - B diag(w) B',  B = Sigma^-1 E   (chunks of up to 1024 columns, as in the _cols
+//                 gradient, into the lower and upper tiles of one m_pad x m_pad buffer Ws),  mubar = B w,  Ybar* = -B diag(w)
+//   -Kbar_sx    = -[Ws mubar] [P alpha]'          (tile GEMM, K = m_pad + 1)
+//   -2 Cbar     = P Kbar_sx + alpha beta' = -[P alpha] [-Kbar_sx; -beta']   (lower tiles, K = m_pad + 1),  beta = P mubar
+// The three blocks are the lower triangle of one symmetric W over the stacked points [x (n_pad rows); x* (m_pad rows)]:
+// the objective's kernel terms are <Cbar, K_xx> + <Kbar_sx, K_sx> + <Sigmabar, K_ss> = 1/2 <W, K([x; x*])> with
+// W = [2 Cbar, Kbar_xs; Kbar_sx, 2 Sigmabar], so grad_reductions_on with alpha = 0 and -W in place of C^-1 gives the
+// hyper-parameters, the noise diagonals (1/2 W_ii: Cbar_ii, then Sigmabar_mm) and both input gradients in one pass of
+// the existing reductions.  Padding rows of either block have zero rows and columns in W and add nothing.  The -beta'
+// row sits in XK extra rows under the stacked buffer so that the K = m_pad + 1 product reads it from the same operand.
+// Why this and not a rectangular reduction over Kbar_sx (or, for single kernels, vfe_cross_grad_kernel +
+// vfe_x_grad_kernel with isn = 1, delta = alpha, r = mubar): the stacked pass visits the same pairs, N^2/2 + NM + M^2/2,
+// with kernels that are already validated for every family, transform and composite descriptor, both dtypes and both
+// layouts, so it needs no new kernel, no float instantiation of the VFE ones and no second copy of the composite
+// derivative rules; the VFE kernels take the square sums only from their own K_zz pass and would still need grad_x and
+// grad_reduce for K_xx and K_ss.  Its cost is memory: the stacked buffer holds the 2 NM elements of the unused upper block
+// besides the blocks.  V, A, the factor of Sigma and Vs are freed before it is allocated, so the peak is about
+// (N + M)^2 + NM + M^2 elements of T (W, P, Ws) besides the handle (agp.h).
+template <typename T>
+int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp_mean* mean_s,
+                               const agp_noise* noise_s, const void* Ys, int S, const double* lp_bar, void* lp_out,
+                               double* grad_out, void* noise_diag_out, void* mean_diag_out, void* y_bar_out, void* x_grad_out,
+                               void* noise_s_diag_out, void* mean_s_diag_out, void* ys_bar_out, void* xs_grad_out) {
+  agp_ctx* ctx = p->ctx;
+  if (S < 1) { ctx->err = "S must be >= 1"; return AGP_ERR_INVALID; }
+  if (!Ys) { ctx->err = "Ys is NULL"; return AGP_ERR_INVALID; }
+  if (!Xs) { ctx->err = "Xs is NULL"; return AGP_ERR_INVALID; }
+  if (M <= 0) { ctx->err = "M must be positive"; return AGP_ERR_DIM_MISMATCH; }
+  static const agp_noise default_noise{0, 1e-18, nullptr};  // default_sigma^2, as agp_post_logpdf
+  if (!noise_s) noise_s = &default_noise;
+  if (noise_s->kind == 1 && !noise_s->v) { ctx->err = "noise vector is NULL"; return AGP_ERR_INVALID; }
+  agp_mean mz{p->mean_kind, p->mean_c, nullptr};
+  if (!mean_s) mean_s = &mz;
+  if (mean_s->kind == 2 && !mean_s->v) { ctx->err = "mean vector is NULL"; return AGP_ERR_INVALID; }
+  int rc = logpdf_grad_prelude<T>(p, layout);
+  if (rc) return rc;
+  cudaStream_t s = ctx->stream;
+  const int64_t N = p->n, n_pad = p->n_pad, m_pad = round_up(M, TILE), ldf = m_pad + TILE;
+  const int D = p->D, nblk = (int)(m_pad / TILE);
+  constexpr int64_t XK = 16;  // extra product columns: [.. alpha], [.. mubar], the -beta' row (one used, 16 keeps alignment)
+  const bool want_red = grad_out || noise_diag_out || x_grad_out || noise_s_diag_out || xs_grad_out;
+  const bool want_beta = want_red || mean_diag_out || y_bar_out;
+  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  Scratch sc(ctx);
+  void* tmp = nullptr;
+
+  // ---- forward: mu*, A = L^-1 K_xs, Sigma = K_ss + Sigma* - A'A and its factor (post_cond_impl's)
+  T *Xst = nullptr, *A = nullptr;
+  rc = post_cross<T>(p, sc, layout, Xs, M, m_pad, &Xst, &A);
+  if (rc) return rc;
+  T *mean_d = nullptr, *noise_d = nullptr;
+  if (mean_s->kind == 2) { rc = upload<T>(ctx, sc, mean_s->v, M, true, &mean_d); if (rc) return rc; }
+  if (noise_s->kind == 1) { rc = upload<T>(ctx, sc, noise_s->v, M, true, &noise_d); if (rc) return rc; }
+  CK(sc.alloc(&tmp, (size_t)m_pad * sizeof(T)));
+  T* mu = (T*)tmp;
+  CK(cudaMemsetAsync(mu, 0, (size_t)m_pad * sizeof(T), s));
+  launch_gemv_t<T>(A, n_pad, n_pad, M, (const T*)p->alpha, mean_s->kind, mean_s->c, mean_d, mu, s);
+  forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, A, n_pad, m_pad);
+  CK(sc.alloc(&tmp, (size_t)ldf * m_pad * sizeof(T)));
+  T* Lf = (T*)tmp;
+  CK(sc.alloc(&tmp, (size_t)nblk * TILE * TILE * sizeof(T)));
+  T* Dinv = (T*)tmp;
+  {
+    GramParams gp{};
+    fill_gram_params<T>(gp, &p->k, 1, 1, M, M, noise_s, noise_d, p->comp);
+    launch_gram<T>(Xst, Xst, m_pad, m_pad, D, Lf, ldf, gp, s);
+    GemmArgs g{};
+    g.A = A; g.lda = n_pad; g.a_kmajor = 1;
+    g.B = A; g.ldb = n_pad; g.b_kmajor = 1;
+    g.C = Lf; g.ldc = ldf; g.M = m_pad; g.N = m_pad; g.K = n_pad;
+    g.alpha_neg = 1; g.beta_one = 1; g.lower_only = 1;
+    launch_gemm<T>(g, s);
+  }
+  launch_border_init<T>(Lf, ldf, M, m_pad, (const T*)nullptr, M, 0, 0, 0.0, (const T*)nullptr, s);
+  CK(sc.alloc(&tmp, (size_t)(nblk + TILE + 2) * sizeof(double)));
+  double* dscal = (double*)tmp;
+  CK(sc.alloc(&tmp, sizeof(int)));
+  int* dinfo = (int*)tmp;
+  CK(cudaMemsetAsync(dinfo, 0, sizeof(int), s));
+  prof_begin(ctx);
+  cholesky_inplace<T>(ctx, Lf, ldf, m_pad, ldf, Dinv, dscal, dinfo);
+  int h_info = 0;
+  std::vector<double> hld((size_t)nblk);
+  CK(cudaMemcpyAsync(&h_info, dinfo, sizeof(int), cudaMemcpyDeviceToHost, s));
+  CK(cudaMemcpyAsync(hld.data(), dscal, (size_t)nblk * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  if (h_info != 0) {
+    ctx->info = h_info;
+    char b[128];
+    snprintf(b, sizeof(b), "posterior covariance is not positive definite; Cholesky failed at pivot %d", h_info);
+    ctx->err = b;
+    return AGP_ERR_NOT_POSDEF;
+  }
+  double logdet = 0.0;
+  for (double v : hld) logdet += v;
+  logdet *= 2.0;
+
+  // ---- Sigma^-1 = Vs'Vs (Vs = L*^-1 with its identity padding zeroed, so nothing outside M x M is nonzero), then the
+  // columns: Ws = -2 Sigmabar, mubar (column m_pad of Ws), Ybar*, and the squared Mahalanobis norms for the values
+  CK(sc.alloc(&tmp, (size_t)m_pad * m_pad * sizeof(T)));
+  T* Vs = (T*)tmp;
+  CK(cudaMemsetAsync(Vs, 0, (size_t)m_pad * m_pad * sizeof(T), s));
+  launch_add_diag<T>(Vs, m_pad, M, 1.0, s);
+  forward_subst_multi<T>(ctx, (const T*)Lf, ldf, (const T*)Dinv, m_pad, Vs, m_pad, m_pad);
+  CK(sc.alloc(&tmp, (size_t)m_pad * (m_pad + XK) * sizeof(T)));
+  T* Ws = (T*)tmp;
+  T* mubar = Ws + m_pad * m_pad;
+  CK(cudaMemsetAsync(Ws, 0, (size_t)m_pad * (m_pad + XK) * sizeof(T), s));
+  std::vector<double> w((size_t)S, 1.0);
+  if (lp_bar) w.assign(lp_bar, lp_bar + S);
+  double wsum = 0.0;
+  for (double v : w) wsum += v;
+  if (want_red) {
+    GemmArgs g{};  // (sum w) Sigma^-1, both triangles
+    g.A = Vs; g.lda = m_pad; g.a_kmajor = 1;
+    g.B = Vs; g.ldb = m_pad; g.b_kmajor = 1;
+    g.C = Ws; g.ldc = m_pad; g.M = m_pad; g.N = m_pad; g.K = m_pad;
+    launch_gemm<T>(g, s);
+    if (wsum != 1.0) launch_scale<T>(Ws, m_pad * m_pad, wsum, s);
+  }
+  std::vector<T> hw((size_t)2 * S);  // w, then -w
+  for (int j = 0; j < S; ++j) { hw[(size_t)j] = (T)w[(size_t)j]; hw[(size_t)S + j] = (T)-w[(size_t)j]; }
+  T* wd = nullptr;
+  rc = upload<T>(ctx, sc, hw.data(), hw.size(), true, &wd);
+  if (rc) return rc;
+  CK(sc.alloc(&tmp, (size_t)S * sizeof(T)));
+  T* sq = (T*)tmp;
+  CK(cudaMemsetAsync(sq, 0, (size_t)S * sizeof(T), s));
+  const int64_t chunk = 1024, cmax = round_up(S < chunk ? S : chunk, TILE);
+  CK(sc.alloc(&tmp, (size_t)m_pad * cmax * sizeof(T) * 2));
+  T* Bc = (T*)tmp;  // E_c, L*^-1 E_c, then Ybar*_c
+  T* Ac = Bc + m_pad * cmax;
+  for (int64_t c0 = 0; c0 < S; c0 += chunk) {
+    const int64_t nc = (S - c0 < chunk) ? (S - c0) : chunk, nc_pad = round_up(nc, TILE);
+    Scratch scc(ctx);
+    T* Yd = nullptr;
+    rc = upload<T>(ctx, scc, (const T*)Ys + (size_t)c0 * M, (size_t)M * nc, false, &Yd);
+    if (rc) return rc;
+    launch_sub_mean_cols<T>(Yd, M, M, nc, 2, 0.0, mu, Bc, m_pad, m_pad, nc_pad, s);
+    forward_subst_multi<T>(ctx, (const T*)Lf, ldf, (const T*)Dinv, m_pad, Bc, m_pad, nc_pad);
+    launch_colsumsq_acc<T>(Bc, m_pad, M, nc, 1.0, sq + c0, s);
+    {
+      GemmArgs g{};  // B_c = Vs' (L*^-1 E_c)
+      g.A = Vs; g.lda = m_pad; g.a_kmajor = 1;
+      g.B = Bc; g.ldb = m_pad; g.b_kmajor = 1;
+      g.C = Ac; g.ldc = m_pad; g.M = m_pad; g.N = nc_pad; g.K = m_pad;
+      launch_gemm<T>(g, s);
+    }
+    launch_gemv_n_acc<T>(Ac, m_pad, M, nc, wd + c0, mubar, s);
+    CK(cudaMemcpyAsync(Bc, Ac, (size_t)m_pad * nc_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    launch_scale_cols<T>(Bc, m_pad, m_pad, nc, wd + S + c0, s);  // Ybar*_c = B_c diag(-w_c)
+    if (want_red) {
+      GemmArgs g{};  // Ws += Ybar*_c B_c', both triangles
+      g.A = Bc; g.lda = m_pad; g.a_kmajor = 0;
+      g.B = Ac; g.ldb = m_pad; g.b_kmajor = 0;
+      g.C = Ws; g.ldc = m_pad; g.M = m_pad; g.N = m_pad; g.K = nc_pad; g.beta_one = 1;
+      launch_gemm<T>(g, s);
+    }
+    if (ys_bar_out)
+      CK(cudaMemcpy2DAsync((T*)ys_bar_out + (size_t)c0 * M, (size_t)M * sizeof(T), Bc, (size_t)m_pad * sizeof(T),
+                           (size_t)M * sizeof(T), (size_t)nc, kout, s));
+  }
+  if (lp_out) {  // logpdf_s = -1/2 (M log 2 pi + logdet Sigma + |L*^-1 e_s|^2)
+    std::vector<T> h((size_t)S);
+    CK(cudaMemcpyAsync(h.data(), sq, (size_t)S * sizeof(T), cudaMemcpyDeviceToHost, s));
+    CK(cudaStreamSynchronize(s));
+    const double log2pi = 1.8378770664093454835606594728112;
+    for (int j = 0; j < S; ++j) h[(size_t)j] = (T)(-0.5 * ((double)M * log2pi + logdet + (double)h[(size_t)j]));
+    CK(cudaMemcpyAsync(lp_out, h.data(), (size_t)S * sizeof(T),
+                       ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyHostToDevice : cudaMemcpyHostToHost, s));
+    CK(cudaStreamSynchronize(s));
+  }
+  rc = download<T>(ctx, mean_s_diag_out, mubar, (size_t)M, false);
+  if (rc) return rc;
+  // buffers are returned to the pool as soon as they are dead (stream-ordered), so that V and the stacked W are never
+  // live together
+  auto drop = [&](void* q) { sc.release(q); cudaFreeAsync(q, s); };
+  drop(Vs); drop(Lf); drop(Dinv);
+
+  // ---- training side: P = V'A with alpha in its column m_pad, beta = P mubar
+  if (want_beta) {
+    T *V = nullptr, *unused = nullptr;
+    rc = inverse_factor<T>(p, sc, false, &V, &unused);
+    if (rc) return rc;
+    CK(sc.alloc(&tmp, (size_t)n_pad * (m_pad + XK) * sizeof(T)));
+    T* P = (T*)tmp;
+    CK(cudaMemsetAsync(P + n_pad * m_pad, 0, (size_t)n_pad * XK * sizeof(T), s));
+    {
+      GemmArgs g{};
+      g.A = V; g.lda = n_pad; g.a_kmajor = 1;
+      g.B = A; g.ldb = n_pad; g.b_kmajor = 1;
+      g.C = P; g.ldc = n_pad; g.M = n_pad; g.N = m_pad; g.K = n_pad;
+      launch_gemm<T>(g, s);
+    }
+    drop(V); drop(A);
+    CK(cudaMemcpyAsync(P + n_pad * m_pad, p->alpha, (size_t)N * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    CK(sc.alloc(&tmp, (size_t)n_pad * 2 * sizeof(T)));
+    T* beta = (T*)tmp;
+    T* nbeta = beta + n_pad;
+    CK(cudaMemsetAsync(beta, 0, (size_t)n_pad * 2 * sizeof(T), s));
+    launch_gemv_n_acc<T>(P, n_pad, N, M, mubar, beta, s);
+    CK(cudaMemcpyAsync(nbeta, beta, (size_t)n_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    launch_scale<T>(nbeta, n_pad, -1.0, s);
+    rc = download<T>(ctx, y_bar_out, beta, (size_t)N, false);
+    if (rc) return rc;
+    rc = download<T>(ctx, mean_diag_out, nbeta, (size_t)N, false);
+    if (rc) return rc;
+    if (want_red) {
+      const int64_t Lst = n_pad + m_pad, ldw = Lst + XK;
+      CK(sc.alloc(&tmp, (size_t)ldw * Lst * sizeof(T)));
+      T* Wst = (T*)tmp;
+      {
+        GemmArgs g{};  // -Kbar_sx = -[Ws mubar][P alpha]' into rows n_pad.. of the first n_pad columns
+        g.A = Ws; g.lda = m_pad; g.a_kmajor = 0;
+        g.B = P; g.ldb = n_pad; g.b_kmajor = 0;
+        g.C = Wst + n_pad; g.ldc = ldw; g.M = m_pad; g.N = n_pad; g.K = m_pad + XK; g.alpha_neg = 1;
+        launch_gemm<T>(g, s);
+      }
+      CK(cudaMemset2DAsync(Wst + Lst, (size_t)ldw * sizeof(T), 0, (size_t)XK * sizeof(T), (size_t)n_pad, s));
+      CK(cudaMemcpy2DAsync(Wst + Lst, (size_t)ldw * sizeof(T), nbeta, sizeof(T), sizeof(T), (size_t)n_pad,
+                           cudaMemcpyDeviceToDevice, s));  // the -beta' row under -Kbar_sx
+      {
+        GemmArgs g{};  // -2 Cbar = -[P alpha][-Kbar_sx; -beta'], lower tiles
+        g.A = P; g.lda = n_pad; g.a_kmajor = 0;
+        g.B = Wst + n_pad; g.ldb = ldw; g.b_kmajor = 1;
+        g.C = Wst; g.ldc = ldw; g.M = n_pad; g.N = n_pad; g.K = m_pad + XK; g.alpha_neg = 1; g.lower_only = 1;
+        launch_gemm<T>(g, s);
+      }
+      launch_copy2d<T>(Ws, m_pad, Wst + n_pad + n_pad * ldw, ldw, m_pad, m_pad, s);  // -2 Sigmabar
+      CK(sc.alloc(&tmp, (size_t)Lst * (D + 1) * sizeof(T)));
+      T* Xcat = (T*)tmp;  // [x; x*] point-major, then alpha = 0
+      T* zalpha = Xcat + Lst * D;
+      CK(cudaMemcpyAsync(Xcat, p->Xt, (size_t)n_pad * D * sizeof(T), cudaMemcpyDeviceToDevice, s));
+      CK(cudaMemcpyAsync(Xcat + n_pad * D, Xst, (size_t)m_pad * D * sizeof(T), cudaMemcpyDeviceToDevice, s));
+      CK(cudaMemsetAsync(zalpha, 0, (size_t)Lst * sizeof(T), s));
+      const bool want_diag = grad_out || noise_diag_out || noise_s_diag_out;
+      const bool want_x = x_grad_out || xs_grad_out;
+      T *nd = nullptr, *xg = nullptr;
+      if (want_diag) { CK(sc.alloc(&tmp, (size_t)Lst * sizeof(T))); nd = (T*)tmp; }
+      if (want_x) { CK(sc.alloc(&tmp, (size_t)Lst * D * sizeof(T))); xg = (T*)tmp; }
+      const bool saved = ctx->out_dev_override;
+      ctx->out_dev_override = true;  // the stacked outputs stay on the device and are split below
+      rc = grad_reductions_on<T>(p, sc, Xcat, Lst, Lst, Wst, ldw, zalpha, grad_out, nd, layout, xg);
+      ctx->out_dev_override = saved;
+      if (rc) return rc;
+      rc = download<T>(ctx, noise_diag_out, nd, (size_t)N, false);
+      if (rc) return rc;
+      rc = download<T>(ctx, noise_s_diag_out, want_diag ? nd + n_pad : nullptr, (size_t)M, false);
+      if (rc) return rc;
+      // the stacked input gradient in `layout`: point-major rows [0, N) and [n_pad, n_pad + M); feature-major columns
+      auto split_x = [&](void* out, int64_t off, int64_t cnt) -> int {
+        if (!out) return AGP_OK;
+        if (layout == AGP_POINT_MAJOR)
+          CK(cudaMemcpyAsync(out, xg + off * D, (size_t)cnt * D * sizeof(T), kout, s));
+        else
+          CK(cudaMemcpy2DAsync(out, (size_t)cnt * sizeof(T), xg + off, (size_t)Lst * sizeof(T), (size_t)cnt * sizeof(T),
+                               (size_t)D, kout, s));
+        return AGP_OK;
+      };
+      rc = split_x(x_grad_out, 0, N);
+      if (rc) return rc;
+      rc = split_x(xs_grad_out, n_pad, M);
+      if (rc) return rc;
+      if (grad_out) {  // d/d sigma^2 = sum_i Cbar_ii and d/d ConstMean c = sum mubar - sum beta, in index order
+        std::vector<T> hn((size_t)N), hb((size_t)N), hm((size_t)M);
+        CK(cudaMemcpyAsync(hn.data(), nd, (size_t)N * sizeof(T), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(hb.data(), beta, (size_t)N * sizeof(T), cudaMemcpyDeviceToHost, s));
+        CK(cudaMemcpyAsync(hm.data(), mubar, (size_t)M * sizeof(T), cudaMemcpyDeviceToHost, s));
+        CK(cudaStreamSynchronize(s));
+        double sn = 0.0, sm = 0.0, sb = 0.0;
+        for (int64_t i = 0; i < N; ++i) { sn += (double)hn[(size_t)i]; sb += (double)hb[(size_t)i]; }
+        for (int64_t i = 0; i < M; ++i) sm += (double)hm[(size_t)i];
+        grad_out[3] = sn;
+        grad_out[4] = sm - sb;
+      }
+    }
   }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
@@ -3131,6 +3424,21 @@ int32_t agp_post_logpdf_grad_cols(agp_post* p, const agp_mean* mean, const void*
                                                     x_grad_out, y_bar_out),
                   post_logpdf_grad_cols_impl<double>(p, mean, Y, S, lp_bar, grad_out, noise_diag_out, mean_diag_out, layout,
                                                      x_grad_out, y_bar_out));
+}
+
+int32_t agp_post_pred_logpdf_grad(agp_post* p, int32_t layout, const void* Xs, int64_t M, const agp_mean* mean_s,
+                                  const agp_noise* noise_s, const void* Ys, int32_t S, const double* lp_bar, void* lp_out,
+                                  double* grad_out, void* noise_diag_out, void* mean_diag_out, void* y_bar_out,
+                                  void* x_grad_out, void* noise_s_diag_out, void* mean_s_diag_out, void* ys_bar_out,
+                                  void* xs_grad_out) {
+  if (!p) return AGP_ERR_INVALID;
+  return DISPATCH(p->dtype,
+                  post_pred_logpdf_grad_impl<float>(p, layout, Xs, M, mean_s, noise_s, Ys, S, lp_bar, lp_out, grad_out,
+                                                    noise_diag_out, mean_diag_out, y_bar_out, x_grad_out, noise_s_diag_out,
+                                                    mean_s_diag_out, ys_bar_out, xs_grad_out),
+                  post_pred_logpdf_grad_impl<double>(p, layout, Xs, M, mean_s, noise_s, Ys, S, lp_bar, lp_out, grad_out,
+                                                     noise_diag_out, mean_diag_out, y_bar_out, x_grad_out, noise_s_diag_out,
+                                                     mean_s_diag_out, ys_bar_out, xs_grad_out));
 }
 
 int32_t agp_post_solve_lower(agp_post* p, const void* B, int64_t nrhs, void* V_out) {

@@ -242,6 +242,52 @@ int32_t agp_post_logpdf_grad_x(agp_post* p, double* grad_out, void* noise_diag_o
 int32_t agp_post_logpdf_grad_cols(agp_post* p, const agp_mean* mean, const void* Y, int32_t S, const double* lp_bar,
                                   double* grad_out, void* noise_diag_out, void* mean_diag_out, int32_t layout,
                                   void* x_grad_out, void* y_bar_out);
+/* The gradient of the held-out log-likelihood of a posterior,
+ *   F = sum_s w_s logpdf(posterior(fx, y)(x*, Sigma*), Y*[:, s]),   w = lp_bar (S host doubles; NULL means ones),
+ * with respect to both sides of the problem: the kernel, the training noise, mean, targets and inputs of the handle, and
+ * the test noise, mean, targets and inputs -- what reverse-mode AD returns through the reference's
+ * logpdf(posterior(fx, y)(x_test, s2), y_test) (examples/0-intro-1d/script.jl's model score).  p must come straight
+ * from agp_fit; y is its target column 0.  With C = K_xx + Sigma_y = L L', delta = y - m, alpha = C^-1 delta,
+ * mu* = m* + K_sx alpha, Sigma = K_ss - K_sx C^-1 K_xs + Sigma*, E = Y* - mu* 1', B = Sigma^-1 E,
+ * P = C^-1 K_xs = V'A (V = L^-1, A = L^-1 K_xs) and beta = P mubar:
+ *   Sigmabar = 1/2 (B diag(w) B' - (sum w) Sigma^-1),  mubar = B w,  Ybar* = -B diag(w)
+ *   Kbar_ss = Sigmabar,  Kbar_sx = mubar alpha' - 2 Sigmabar P' (M x N),  Cbar = Kbar_xx = P Sigmabar P' - 1/2 (beta alpha' + alpha beta')
+ *   ybar = beta,  mbar = -beta at x,  mbar* = mubar,  d/d sigma_i^2 = Cbar_ii,  d/d sigma*_m^2 = Sigmabar_mm,
+ *   d/d ConstMean c = sum mubar - sum beta,  d/d theta = <Cbar, dK_xx> + <Kbar_sx, dK_sx> + <Sigmabar, dK_ss>
+ *   x_grad[i]  = 2 sum_j Cbar_ij d1k(x_i, x_j) + sum_m Kbar_sx[m, i] d2k(x*_m, x_i)
+ *   xs_grad[m] = 2 sum_m' Sigmabar_mm' d1k(x*_m, x*_m') + sum_i Kbar_sx[m, i] d1k(x*_m, x_i)
+ * (d1 / d2 as agp_post_logpdf_grad_x's, through the Scale / ARD chain).  The three kernel blocks are reduced as one
+ * symmetric W = [2 Cbar, Kbar_xs; Kbar_sx, 2 Sigmabar] over the stacked points [x; x*], by the reductions of
+ * agp_post_logpdf_grad_x, so a composite handle is covered as a single kernel is.
+ * Inputs: Xs (M points in `layout`), mean_s (the prior mean at x*, as agp_post_logpdf's; NULL means the handle's zero or
+ * constant mean), noise_s (Sigma*; NULL means 1e-18), Ys (M x S column-major, any S >= 1).
+ * Outputs, each may be NULL and its work is then skipped: lp_out (S values, logpdf of each column), grad_out (double, the
+ * layout of agp_post_logpdf_grad: 5 + D for a single kernel, agp_post_grad_len(p) for a composite; [3] d/d sigma^2 of
+ * the training scalar noise, [4] d/d ConstMean c), noise_diag_out, mean_diag_out and y_bar_out (N values each),
+ * x_grad_out (N x D in `layout`), noise_s_diag_out and mean_s_diag_out (M values each), ys_bar_out (M x S) and
+ * xs_grad_out (M x D in `layout`).  Every output but grad_out has the handle's dtype; under AGP_MEM_DEVICE, Xs, Ys and
+ * those outputs are DEVICE pointers.  The gradient of a scalar test noise is the sum of noise_s_diag_out.
+ * Arithmetic: the handle's dtype for the factors, V, P and the products, fp64 for the reductions (as
+ * agp_post_logpdf_grad_x); the error of fp32 handles grows with cond(C), and the kernel gradient of a Linear prior at
+ * N >> D, a difference of nearly equal terms, can be off by tens of percent in fp32 (DESIGN s6): use an fp64 handle
+ * there.  Cost: the forward of agp_post_logpdf (N^2 M for A, M^3 / 3 for the factor of Sigma), M^3 for
+ * Sigma^-1, 4 M^2 S for the columns, then, when a kernel, noise, x or x* output or one of the training-side outputs is
+ * asked for, ~N^3 for V, 2 N^2 M for P, 2 N M^2 for Kbar_sx, N^2 M for Cbar (the lower half), and the reductions over
+ * (N + M)^2 / 2 pairs.  Memory, besides the handle, in elements of the handle's dtype: about NM + 3 M^2 while Sigma is
+ * factored and inverted, N^2 + 2 NM + M^2 while V is live (V, K_xs / A, P, Sigmabar), then (N + M)^2 + NM + M^2 for the
+ * stacked W (which also holds the 2 NM elements of its unused upper block), P and Sigmabar: each buffer is freed when it
+ * is dead, so the peak is the last.  Add two M x min(S, 1024) chunk buffers.  S goes through in chunks of up to 1024 columns.
+ * Determinism: every per-point output and grad_out[3], grad_out[4] are formed in a fixed order (two calls give the same
+ * bits); the other entries of grad_out leave their CTAs through fp64 atomics and agree to rounding.
+ * Errors: a bad layout, S < 1, a NULL Ys or Xs, or a vector mean / noise with a NULL v: AGP_ERR_INVALID; M < 1:
+ * AGP_ERR_DIM_MISMATCH; an extended handle: AGP_ERR_UNSUPPORTED; a Sigma that is not positive definite:
+ * AGP_ERR_NOT_POSDEF (agp_last_info gives the pivot); a failed device allocation: AGP_ERR_CUDA.  VFE posteriors are not
+ * covered. */
+int32_t agp_post_pred_logpdf_grad(agp_post* p, int32_t layout, const void* Xs, int64_t M, const agp_mean* mean_s,
+                                  const agp_noise* noise_s, const void* Ys, int32_t S, const double* lp_bar, void* lp_out,
+                                  double* grad_out, void* noise_diag_out, void* mean_diag_out, void* y_bar_out,
+                                  void* x_grad_out, void* noise_s_diag_out, void* mean_s_diag_out, void* ys_bar_out,
+                                  void* xs_grad_out);
 /* number of doubles agp_post_logpdf_grad writes: 5 + D for a single kernel, the layout above for a composite */
 int64_t agp_post_grad_len(const agp_post* p);
 /* V = U' \ B (N x nrhs, column-major): backs Xt_invA_X / diag_Xt_invA_X / Xt_invA_Y /

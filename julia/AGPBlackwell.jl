@@ -583,6 +583,87 @@ function CRC.rrule(::typeof(logpdf), fx::DevFiniteGP{T}, Y::AbstractMatrix{<:Rea
     return lp, logpdf_matrix_pullback
 end
 
+# ---- reverse-mode rules for the held-out log-likelihood logpdf(posterior(fx, y)(x*, Σ*), y*) ----------------------------
+# (examples/0-intro-1d/script.jl scores its models with it; validation-likelihood training maximises it.)
+# posterior(fx, y) keeps the handle: its rule runs the primal and its pullback only re-routes a tangent of the DevPosterior
+# -- prior -> fx.f, data.x -> fx.x, data.δ -> y and, since δ = y - m(x), minus its sum to a ConstMean, and data.C -> fx.Σy.
+# logpdf over a DevPosterior makes ONE agp_post_pred_logpdf_grad call with lp_bar = Δ and returns the total derivatives
+# in that tangent shape: the kernel through every block (K_xx, K_xs, K_ss), data.x, data.δ = ȳ, the prior mean through
+# the test side only (the training side reaches it through data.δ), and in data.C the diagonal of the cotangent of
+# C = K_xx + Σy as (noise = its trace, noise_diag = its diagonal): the part of C's cotangent that Σy receives (the kernel
+# part is already in prior.kernel).  Every Tangent names only fields its primal has (FiniteGP: f, x, Σy; GP: mean, kernel;
+# PosteriorGP: prior, data; data: α, C, x, δ).  fx.x, fx.Σy and Y get theirs directly.  A CustomMean closure is not
+# differentiated, as in the rules above.
+notangent(t) = t === nothing || t isa CRC.AbstractZero
+# the c of a ConstMean's tangent as the AD system hands it back (a Tangent or a NamedTuple); 0 for no tangent
+tangent_c(Δm) = notangent(Δm) ? 0.0 : Δm.c
+
+function CRC.rrule(::typeof(posterior), fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T}
+    claimed(fx.f) || return nothing                                       # no rule: AD differentiates the stock method
+    post = posterior(fx, y)
+    function posterior_pullback(Δ)
+        Δp = CRC.unthunk(Δ)
+        notangent(Δp) && return CRC.NoTangent(), CRC.ZeroTangent(), CRC.ZeroTangent()
+        Δd, Δf = Δp.data, Δp.prior
+        ȳ = notangent(Δd) || notangent(Δd.δ) ? zeros(T, length(y)) : Δd.δ
+        # a new ConstMean tangent from the scalar c's, rather than a sum of tangents of different wrappers
+        m̄ = fx.f.mean isa AbstractGPs.ConstMean ?
+            mean_tangent(fx.f.mean, (mean_c=(notangent(Δf) ? 0.0 : tangent_c(Δf.mean)) - sum(ȳ),)) : CRC.NoTangent()
+        f̄ = CRC.Tangent{typeof(fx.f)}(; mean=m̄, kernel=notangent(Δf) ? CRC.NoTangent() : Δf.kernel)
+        x̄ = notangent(Δd) || notangent(Δd.x) ? CRC.NoTangent() : Δd.x
+        Σ̄ = notangent(Δd) || notangent(Δd.C) ? CRC.NoTangent() : noise_tangent(fx.Σy, Δd.C)
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x̄, Σy=Σ̄)
+        return CRC.NoTangent(), f̄x, ȳ
+    end
+    return post, posterior_pullback
+end
+
+# the input gradient comes back in the test points' layout: as the training container's storage
+function as_storage(xg, X, from, to)
+    (X isa AbstractVector || from == to) && return xg
+    return permutedims(xg)
+end
+
+function CRC.rrule(::typeof(logpdf), fx::DevPostFiniteGP{T}, Y::AbstractVecOrMat{<:Real}) where {T}
+    p = fx.f
+    lp = logpdf(fx, Y)
+    c = ctx(); Xs, layout, D = points(fx.x); M = length(fx)
+    X, xlayout, _ = points(p.data.x); N = p.data.C.n
+    Ym = convert(Matrix{T}, reshape(Y, M, :)); S = size(Ym, 2)
+    ms, k2 = mean_spec(p.prior.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
+    composite = !supported(p.prior)
+    function pred_logpdf_pullback(Δ)
+        Δ = CRC.unthunk(Δ)
+        Δ isa CRC.AbstractZero && return CRC.NoTangent(), CRC.ZeroTangent(), CRC.ZeroTangent()
+        w = convert(Vector{Float64}, Δ isa Real ? [Δ] : Δ)
+        glen = composite ? ccall((:agp_post_grad_len, libagp), Int64, (Ptr{Cvoid},), p.data.C.h) : 5 + D
+        g = Vector{Float64}(undef, glen); nd = Vector{T}(undef, N); ȳ = Vector{T}(undef, N)
+        xg = X isa AbstractVector || xlayout == layout ? similar(X, T) : similar(permutedims(X), T)
+        nsd = Vector{T}(undef, M); Ȳ = Matrix{T}(undef, M, S); xsg = similar(Xs, T)
+        lock(c.lock) do
+            GC.@preserve Xs Ym w g nd ȳ xg nsd Ȳ xsg k2 k3 check(c, ccall((:agp_post_pred_logpdf_grad, libagp), Int32,
+                (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Int64, Ref{AgpMean}, Ref{AgpNoise}, Ptr{Cvoid}, Int32, Ptr{Float64}, Ptr{Cvoid},
+                 Ptr{Float64}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                p.data.C.h, layout, Xs, M, ms, ns, Ym, S, w, C_NULL, g, nd, C_NULL, ȳ, xg, nsd, C_NULL, Ȳ, xsg))
+        end
+        # grad_out[5] is d/dc through both sides; the prior mean's tangent keeps the test side, data.δ carries the rest
+        gs = (variance=g[1], scale=g[2], linear_c=g[3], noise=g[4], mean_c=g[5] + sum(ȳ), ard=g[6:end], noise_diag=nd)
+        if composite
+            kt = ctangent(p.prior.kernel, Int[], composite_grads(p.prior.kernel, D, g), 1.0)
+        else
+            _, var, _, wt = flat(p.prior.kernel)
+            kt = kernel_tangent(p.prior.kernel, gs, var, wt === nothing ? 1.0 : wt)
+        end
+        p̄rior = CRC.Tangent{typeof(p.prior)}(; mean=mean_tangent(p.prior.mean, gs), kernel=kt)
+        d̄ata = CRC.Tangent{typeof(p.data)}(; C=(noise=g[4], noise_diag=nd),
+                                            x=x_tangent(p.data.x, as_storage(xg, X, layout, xlayout)), δ=ȳ)
+        f̄ = CRC.Tangent{typeof(p)}(; prior=p̄rior, data=d̄ata)
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, xsg), Σy=noise_tangent(fx.Σy, (noise=sum(nsd), noise_diag=nsd)))
+        return CRC.NoTangent(), f̄x, Y isa AbstractVector ? vec(Ȳ) : Ȳ
+    end
+    return lp, pred_logpdf_pullback
+end
+
 # ---- reverse-mode rule for rand(rng, fx, S) (test/finite_gp_projection.jl:105-127) -----------------------------------
 # The forward pass draws Z exactly as the primal method above and calls agp_rand; the pullback sends the cotangent of the
 # samples through ONE agp_rand_grad call at the same Z (the factor is formed again there).  The tangents reuse the logpdf
