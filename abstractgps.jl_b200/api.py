@@ -898,6 +898,57 @@ def fit(fx: FiniteGP, y):
     return _fit(fx, y, True, True)
 
 
+def _grad_buffer(k: Kernel, D, h=None):
+    """(g, flat): the zeroed gradient vector for kernel k and, for a composite, the _Flat that maps it back onto
+    kernel_params(k) (None otherwise).  With a posterior handle h a composite's length is the handle's."""
+    if not (isinstance(k, _CompositeKernel) or k.family > LINEAR):
+        return np.zeros(5 + D, dtype=np.float64), None
+    flat = _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D)
+    n = int(engine().L.agp_post_grad_len(h)) if h is not None else flat.grad_len()
+    return np.zeros(n, dtype=np.float64), flat
+
+
+def _grad_result(g, flat, k: Kernel, D, mean: "MeanFunction", noise, mean_v):
+    """The gradient dict's kernel, noise and mean keys from g: "kernel" (composite) or "variance", "scale" | "ard",
+    "linear_c"; "noise" (the per-point vector `noise`, else g[3]); "mean_c" (ConstMean) or "mean_v" (CustomMean)."""
+    if flat is not None:
+        res = {"kernel": flat.params_grad(g)}
+    else:
+        res = {"variance": g[0]}
+        if isinstance(k.transform, ScaleTransform):
+            res["scale"] = g[1]
+        elif isinstance(k.transform, ARDTransform):
+            res["ard"] = g[5:5 + D].copy()
+        if k.family == LINEAR:
+            res["linear_c"] = g[2]
+    res["noise"] = g[3] if noise is None else noise.astype(np.float64)
+    if isinstance(mean, ConstMean):
+        res["mean_c"] = g[4]
+    elif isinstance(mean, CustomMean):
+        res["mean_v"] = mean_v.astype(np.float64)
+    return res
+
+
+def _points_grad(kind, n, D, dt):
+    """The buffer a point-major input gradient of n points comes back in, shaped like the container kind: D x n
+    column-major (ColVecs), length n (a vector), or n x D row-major (RowVecs) -- all the same memory order."""
+    return {"col": lambda: np.empty((D, n), dtype=dt, order="F"), "vec": lambda: np.empty(n, dtype=dt),
+            "row": lambda: np.empty((n, D), dtype=dt)}[kind]()
+
+
+def _cols_and_weights(Y, lp_bar, n, dt):
+    """(ndim of Y, Y as an n x S Fortran array, S, lp_bar as float64 or None for all ones)"""
+    Yin = np.asarray(Y)
+    Yf = np.asfortranarray(Yin.reshape(-1, 1) if Yin.ndim == 1 else Yin, dtype=dt)
+    if Yf.shape[0] != n:
+        raise DimensionMismatch("length(fx) = %d but Y has %d rows" % (n, Yf.shape[0]))
+    S = Yf.shape[1]
+    w = None if lp_bar is None else np.ascontiguousarray(lp_bar, dtype=np.float64).ravel()
+    if w is not None and w.shape[0] != S:
+        raise DimensionMismatch("lp_bar has %d entries, Y has %d columns" % (w.shape[0], S))
+    return Yin.ndim, Yf, S, w
+
+
 def logpdf_grad(fx: FiniteGP, y, inputs=False):
     """EXPERIMENTAL (device path not yet validated): (logpdf, gradient dict) of logpdf(fx, y) w.r.t. the kernel variance,
     ScaleTransform s / ARDTransform v, LinearKernel c, the noise (scalar or per-point) and the mean (constant or vector)
@@ -913,38 +964,20 @@ def logpdf_grad(fx: FiniteGP, y, inputs=False):
     dt = post.data.C.dtype
     D = post.data.x.D
     k = f.kernel
-    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
-    g = np.zeros(int(eng.L.agp_post_grad_len(post.data.C.h)) if composite else 5 + D, dtype=np.float64)
+    g, flat = _grad_buffer(k, D, post.data.C.h)
     per_point = np.ndim(fx.s2) != 0
     nd = np.empty(len(fx), dtype=dt) if (per_point or isinstance(f.mean, CustomMean)) else None
     if inputs:
+        # a RowVecs gradient comes back feature-major, N x D column-major like the other containers' memory
         xk = fx.x_kind
-        if xk == "col":
-            layout, xg = cabi.AGP_POINT_MAJOR, np.empty((D, len(fx)), dtype=dt, order="F")
-        elif xk == "vec":
-            layout, xg = cabi.AGP_POINT_MAJOR, np.empty(len(fx), dtype=dt)
-        else:
-            layout, xg = cabi.AGP_FEATURE_MAJOR, np.empty((len(fx), D), dtype=dt, order="F")
+        layout = cabi.AGP_FEATURE_MAJOR if xk == "row" else cabi.AGP_POINT_MAJOR
+        xg = np.empty((len(fx), D), dtype=dt, order="F") if xk == "row" else _points_grad(xk, len(fx), D, dt)
         eng.check(eng.L.agp_post_logpdf_grad_x(post.data.C.h, g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), layout,
                                                cabi.ptr(xg)))
     else:
         eng.check(eng.L.agp_post_logpdf_grad(post.data.C.h, g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd)))
-    if composite:
-        # composite: out["kernel"][i] is the derivative in kernel_params(k)[i] (the descriptor's gradient mapped back)
-        out = {"kernel": _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D).params_grad(g)}
-    else:
-        out = {"variance": g[0]}
-        if isinstance(k.transform, ScaleTransform):
-            out["scale"] = g[1]
-        elif isinstance(k.transform, ARDTransform):
-            out["ard"] = g[5:5 + D].copy()
-        if k.family == LINEAR:
-            out["linear_c"] = g[2]
-    out["noise"] = nd.astype(np.float64) if per_point else g[3]
-    if isinstance(f.mean, ConstMean):
-        out["mean_c"] = g[4]
-    elif isinstance(f.mean, CustomMean):
-        out["mean_v"] = post.data.alpha.astype(np.float64)
+    # composite: out["kernel"][i] is the derivative in kernel_params(k)[i] (the descriptor's gradient mapped back)
+    out = _grad_result(g, flat, k, D, f.mean, nd if per_point else None, post.data.alpha)
     if inputs:
         out["x"] = xg
     return lp, out
@@ -963,53 +996,27 @@ def loglikelihood_grad(fx: FiniteGP, Y, lp_bar=None, inputs=False):
     if not isinstance(fx.f, GP):
         raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "the gradient of logpdf over a matrix Y is implemented for a FiniteGP over "
                        "a prior GP, not over %s" % type(fx.f).__name__)
-    Yin = np.asarray(Y)
     dt = fx.dtype
     pts = fx.x.astype(dt)
     N, D = pts.n, pts.D
-    Yf = np.asfortranarray(Yin.reshape(-1, 1) if Yin.ndim == 1 else Yin, dtype=dt)
-    if Yf.shape[0] != N:
-        raise DimensionMismatch("length(fx) = %d but Y has %d rows" % (N, Yf.shape[0]))
-    S = Yf.shape[1]
-    w = None if lp_bar is None else np.ascontiguousarray(lp_bar, dtype=np.float64).ravel()  # None: all ones
-    if w is not None and w.shape[0] != S:
-        raise DimensionMismatch("lp_bar has %d entries, Y has %d columns" % (w.shape[0], S))
+    ndim, Yf, S, w = _cols_and_weights(Y, lp_bar, N, dt)
     lp, post = _fit(fx, Yf, True, False)
     eng = engine()
     f = fx.f
     k = f.kernel
-    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
-    flat = _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D) if composite else None
-    g = np.zeros(flat.grad_len() if composite else 5 + D, dtype=np.float64)
-    per_point = np.ndim(fx.s2) != 0
-    nd = np.empty(N, dtype=dt) if per_point else None
+    g, flat = _grad_buffer(k, D)
+    nd = np.empty(N, dtype=dt) if np.ndim(fx.s2) != 0 else None
     md = np.empty(N, dtype=dt) if isinstance(f.mean, CustomMean) else None
     yb = np.empty((N, S), dtype=dt, order="F")
-    # the points go in point-major, so x comes back point-major: D x N column-major, i.e. N x D row-major
-    xg = {"col": lambda: np.empty((D, N), dtype=dt, order="F"), "vec": lambda: np.empty(N, dtype=dt),
-          "row": lambda: np.empty((N, D), dtype=dt)}[fx.x_kind]() if inputs else None
+    xg = _points_grad(fx.x_kind, N, D, dt) if inputs else None  # the points go in point-major
     keep = []
     ms = _mean_struct(f.mean.spec(pts, dt), keep)
     eng.check(eng.L.agp_post_logpdf_grad_cols(post.data.C.h, C.byref(ms), cabi.ptr(Yf), S,
                                               None if w is None else w.ctypes.data_as(C.POINTER(C.c_double)),
                                               g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), cabi.ptr(md),
                                               cabi.AGP_POINT_MAJOR, cabi.ptr(xg), cabi.ptr(yb)))
-    if composite:
-        res = {"kernel": flat.params_grad(g)}
-    else:
-        res = {"variance": g[0]}
-        if isinstance(k.transform, ScaleTransform):
-            res["scale"] = g[1]
-        elif isinstance(k.transform, ARDTransform):
-            res["ard"] = g[5:5 + D].copy()
-        if k.family == LINEAR:
-            res["linear_c"] = g[2]
-    res["noise"] = nd.astype(np.float64) if per_point else g[3]
-    if isinstance(f.mean, ConstMean):
-        res["mean_c"] = g[4]
-    elif isinstance(f.mean, CustomMean):
-        res["mean_v"] = md.astype(np.float64)
-    res["Y"] = yb[:, 0].copy() if Yin.ndim == 1 else yb
+    res = _grad_result(g, flat, k, D, f.mean, nd, md)
+    res["Y"] = yb[:, 0].copy() if ndim == 1 else yb
     if inputs:
         res["x"] = xg
     return np.atleast_1d(lp), res
@@ -1034,18 +1041,10 @@ def posterior_logpdf_grad(fx: FiniteGP, Y, lp_bar=None, inputs=False):
     p, dt, pts, ms, ns, keep = _post_args(fx)
     fx0 = p.fx
     N, M, D = p.data.x.n, pts.n, pts.D
-    Yin = np.asarray(Y)
-    Yf = np.asfortranarray(Yin.reshape(-1, 1) if Yin.ndim == 1 else Yin, dtype=dt)
-    if Yf.shape[0] != M:
-        raise DimensionMismatch("length(fx) = %d but Y has %d rows" % (M, Yf.shape[0]))
-    S = Yf.shape[1]
-    w = None if lp_bar is None else np.ascontiguousarray(lp_bar, dtype=np.float64).ravel()  # None: all ones
-    if w is not None and w.shape[0] != S:
-        raise DimensionMismatch("lp_bar has %d entries, Y has %d columns" % (w.shape[0], S))
+    ndim, Yf, S, w = _cols_and_weights(Y, lp_bar, M, dt)
     f = p.prior
     k = f.kernel
-    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
-    g = np.zeros(int(eng.L.agp_post_grad_len(p.data.C.h)) if composite else 5 + D, dtype=np.float64)
+    g, flat = _grad_buffer(k, D, p.data.C.h)
     lp = np.empty(S, dtype=dt)
     nd = np.empty(N, dtype=dt) if np.ndim(fx0.s2) != 0 else None
     md = np.empty(N, dtype=dt) if isinstance(f.mean, CustomMean) else None
@@ -1053,39 +1052,22 @@ def posterior_logpdf_grad(fx: FiniteGP, Y, lp_bar=None, inputs=False):
     nsd = np.empty(M, dtype=dt)
     msd = np.empty(M, dtype=dt) if isinstance(f.mean, CustomMean) else None
     ysb = np.empty((M, S), dtype=dt, order="F")
-    # the points go in point-major, so the input gradients come back point-major: D x n column-major, n x D row-major
-    shape = lambda kind, n: {"col": lambda: np.empty((D, n), dtype=dt, order="F"), "vec": lambda: np.empty(n, dtype=dt),
-                             "row": lambda: np.empty((n, D), dtype=dt)}[kind]()
-    xg = shape(fx0.x_kind, N) if inputs else None
-    xsg = shape(fx.x_kind, M) if inputs else None
+    xg = _points_grad(fx0.x_kind, N, D, dt) if inputs else None  # the points go in point-major
+    xsg = _points_grad(fx.x_kind, M, D, dt) if inputs else None
     dbl = lambda a: None if a is None else a.ctypes.data_as(C.POINTER(C.c_double))
     eng.check(eng.L.agp_post_pred_logpdf_grad(p.data.C.h, cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), M, C.byref(ms), C.byref(ns),
                                               cabi.ptr(Yf), S, dbl(w), cabi.ptr(lp), dbl(g), cabi.ptr(nd), cabi.ptr(md),
                                               cabi.ptr(yb), cabi.ptr(xg), cabi.ptr(nsd), cabi.ptr(msd), cabi.ptr(ysb),
                                               cabi.ptr(xsg)))
-    if composite:
-        res = {"kernel": _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D).params_grad(g)}
-    else:
-        res = {"variance": g[0]}
-        if isinstance(k.transform, ScaleTransform):
-            res["scale"] = g[1]
-        elif isinstance(k.transform, ARDTransform):
-            res["ard"] = g[5:5 + D].copy()
-        if k.family == LINEAR:
-            res["linear_c"] = g[2]
-    res["noise"] = nd.astype(np.float64) if nd is not None else g[3]
-    if isinstance(f.mean, ConstMean):
-        res["mean_c"] = g[4]
-    elif isinstance(f.mean, CustomMean):
-        res["mean_v"] = md.astype(np.float64)
+    res = _grad_result(g, flat, k, D, f.mean, nd, md)
     res["y"] = yb
     res["noise_s"] = nsd.astype(np.float64) if np.ndim(fx.s2) != 0 else float(np.sum(nsd, dtype=np.float64))
     if msd is not None:
         res["mean_s_v"] = msd.astype(np.float64)
-    res["Y"] = ysb[:, 0].copy() if Yin.ndim == 1 else ysb
+    res["Y"] = ysb[:, 0].copy() if ndim == 1 else ysb
     if inputs:
         res["x"], res["xs"] = xg, xsg
-    return (lp[0] if Yin.ndim == 1 else lp), res
+    return (lp[0] if ndim == 1 else lp), res
 
 
 def _post_call(p: PosteriorGP, pts: _Points, s2, want_var=True, want_cov=False):
@@ -1337,35 +1319,16 @@ def rand_grad(fx: FiniteGP, Z, out_bar, inputs=False):
     ms = _mean_struct(f.mean.spec(pts, dt), keep)
     ns = _noise_struct(fx.s2, N, dt, keep)
     k = f.kernel
-    composite = isinstance(k, _CompositeKernel) or k.family > LINEAR
-    flat = _Flat(k if isinstance(k, _CompositeKernel) else KernelSum(k), D) if composite else None
-    g = np.zeros(flat.grad_len() if composite else 5 + D, dtype=np.float64)
-    per_point = np.ndim(fx.s2) != 0
-    nd = np.empty(N, dtype=dt) if per_point else None
+    g, flat = _grad_buffer(k, D)
+    nd = np.empty(N, dtype=dt) if np.ndim(fx.s2) != 0 else None
     md = np.empty(N, dtype=dt) if isinstance(f.mean, CustomMean) else None
     zb = np.empty((N, S), dtype=dt, order="F")
-    # the points go in point-major, so x comes back point-major: D x N column-major, i.e. N x D row-major
-    xg = {"col": lambda: np.empty((D, N), dtype=dt, order="F"), "vec": lambda: np.empty(N, dtype=dt),
-          "row": lambda: np.empty((N, D), dtype=dt)}[fx.x_kind]() if inputs else None
+    xg = _points_grad(fx.x_kind, N, D, dt) if inputs else None  # the points go in point-major
     eng.check(eng.L.agp_rand_grad(eng.h, cabi.dtype_code(dt), C.byref(ks), C.byref(ms), C.byref(ns), cabi.AGP_POINT_MAJOR,
                                   cabi.ptr(pts.a), N, D, cabi.ptr(Zf), S, cabi.ptr(Of),
                                   g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), cabi.ptr(md), cabi.ptr(xg),
                                   cabi.ptr(zb)))
-    if composite:
-        res = {"kernel": flat.params_grad(g)}
-    else:
-        res = {"variance": g[0]}
-        if isinstance(k.transform, ScaleTransform):
-            res["scale"] = g[1]
-        elif isinstance(k.transform, ARDTransform):
-            res["ard"] = g[5:5 + D].copy()
-        if k.family == LINEAR:
-            res["linear_c"] = g[2]
-    res["noise"] = nd.astype(np.float64) if per_point else g[3]
-    if isinstance(f.mean, ConstMean):
-        res["mean_c"] = g[4]
-    elif isinstance(f.mean, CustomMean):
-        res["mean_v"] = md.astype(np.float64)
+    res = _grad_result(g, flat, k, D, f.mean, nd, md)
     res["Z"] = zb.reshape(Zin.shape) if Zin.ndim == 1 else zb
     if inputs:
         res["x"] = xg
@@ -1487,35 +1450,20 @@ def approx_log_evidence_grad(vfe: VFE, fx: FiniteGP, y, inputs=False):
     if isinstance(k, _CompositeKernel) or k.family > LINEAR:
         raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "composite kernels are supported on the exact path only (not VFE)")
     value = np.empty(1, dtype=dt)
-    g = np.zeros(5 + D, dtype=np.float64)
-    per_point = np.ndim(fx.s2) != 0
-    nd = np.empty(pts.n, dtype=dt) if per_point else None
+    g, flat = _grad_buffer(k, D)
+    nd = np.empty(pts.n, dtype=dt) if np.ndim(fx.s2) != 0 else None
     md = np.empty(pts.n, dtype=dt) if isinstance(f.mean, CustomMean) else None
-    # the points go in point-major, so z comes back point-major: D x M column-major, i.e. M x D row-major
-    zg = {"col": lambda: np.empty((D, z.n), dtype=dt, order="F"), "vec": lambda: np.empty(z.n, dtype=dt),
-          "row": lambda: np.empty((z.n, D), dtype=dt)}[vfe.fz.x_kind]()
+    zg = _points_grad(vfe.fz.x_kind, z.n, D, dt)  # the points go in point-major
     objective = 1 if isinstance(vfe, DTC) else 0
     args = (eng.h, cabi.dtype_code(dt), C.byref(ks), C.byref(ms), C.byref(ns), cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), pts.n,
             pts.D, cabi.ptr(z.a), z.n, C.byref(js), cabi.ptr(y), objective, cabi.ptr(value),
             g.ctypes.data_as(C.POINTER(C.c_double)), cabi.ptr(nd), cabi.ptr(md), cabi.ptr(zg))
-    if inputs:  # point-major like z: D x N column-major, i.e. N x D row-major
-        xg = {"col": lambda: np.empty((D, pts.n), dtype=dt, order="F"), "vec": lambda: np.empty(pts.n, dtype=dt),
-              "row": lambda: np.empty((pts.n, D), dtype=dt)}[fx.x_kind]()
+    if inputs:
+        xg = _points_grad(fx.x_kind, pts.n, D, dt)
         eng.check(eng.L.agp_vfe_elbo_grad_x(*args, cabi.ptr(xg)))
     else:
         eng.check(eng.L.agp_vfe_elbo_grad(*args))
-    out = {"variance": g[0]}
-    if isinstance(k.transform, ScaleTransform):
-        out["scale"] = g[1]
-    elif isinstance(k.transform, ARDTransform):
-        out["ard"] = g[5:5 + D].copy()
-    if k.family == LINEAR:
-        out["linear_c"] = g[2]
-    out["noise"] = nd.astype(np.float64) if per_point else g[3]
-    if isinstance(f.mean, ConstMean):
-        out["mean_c"] = g[4]
-    elif isinstance(f.mean, CustomMean):
-        out["mean_v"] = md.astype(np.float64)
+    out = _grad_result(g, flat, k, D, f.mean, nd, md)
     out["z"] = zg
     if inputs:
         out["x"] = xg

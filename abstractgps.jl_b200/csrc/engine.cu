@@ -1091,6 +1091,76 @@ int post_mean_cov_impl(agp_post* p, int layout, const void* Xs, int64_t M, const
 // mean_and_cov is /root/reference/src/exact_gpr_posterior.jl:78-83).  The M x M posterior covariance never
 // leaves the device: K** + Sigma* is generated straight into a factor buffer, V'V (V = L^-1 K(x, x*)) is
 // subtracted by one GEMM, and the same in-place Cholesky as agp_fit runs with (Y - m*)' in the border tile.
+
+// the test-side defaults of agp_post_logpdf / agp_post_rand / agp_post_pred_logpdf_grad: the handle's mean, and
+// default_sigma^2 (finite_gp_projection.jl:17) for the noise.  handle_mean holds the default mean for the call.
+inline int post_side_defaults(agp_post* p, const agp_mean** mean_s, const agp_noise** noise_s, agp_mean* handle_mean) {
+  agp_ctx* ctx = p->ctx;
+  static const agp_noise default_noise{0, 1e-18, nullptr};
+  if (!*noise_s) *noise_s = &default_noise;
+  if ((*noise_s)->kind == 1 && !(*noise_s)->v) { ctx->err = "noise vector is NULL"; return AGP_ERR_INVALID; }
+  *handle_mean = agp_mean{p->mean_kind, p->mean_c, nullptr};
+  if (!*mean_s) *mean_s = handle_mean;
+  if ((*mean_s)->kind == 2 && !(*mean_s)->v) { ctx->err = "mean vector is NULL"; return AGP_ERR_INVALID; }
+  return AGP_OK;
+}
+
+// C* + Sigma* = K(x*, x*) + Sigma* - A'A (A = L^-1 K(x, x*), the handle's n_pad rows), lower triangle, with (Y - mu)' in
+// the border (S columns; none with S = 0), factored in place by agp_fit's Cholesky.  Into the call's scratch: Lf_out the
+// factor (leading dimension m_pad + TILE, identity padding), Dinv_out its inverted diagonal blocks, dscal_out the
+// per-block log-determinants (then the border's sums), dinfo_out the failed pivot (read by post_cov_status).
+template <typename T>
+int post_cov_factor(agp_post* p, Scratch& sc, const T* Xst, const T* A, int64_t M, const agp_noise* noise_s,
+                    const T* noise_d, const T* Yd, int S, const T* mu, T** Lf_out, T** Dinv_out, double** dscal_out,
+                    int** dinfo_out) {
+  agp_ctx* ctx = p->ctx;
+  cudaStream_t s = ctx->stream;
+  const int64_t m_pad = round_up(M, TILE), ldf = m_pad + TILE;
+  const int nblk = (int)(m_pad / TILE);
+  void* tmp = nullptr;
+  CK(sc.alloc(&tmp, (size_t)ldf * m_pad * sizeof(T)));
+  T* Lf = (T*)tmp;
+  CK(sc.alloc(&tmp, (size_t)nblk * TILE * TILE * sizeof(T)));
+  T* Dinv = (T*)tmp;
+  GramParams gp{};
+  fill_gram_params<T>(gp, &p->k, 1, 1, M, M, noise_s, noise_d, p->comp);
+  launch_gram<T>(Xst, Xst, m_pad, m_pad, p->D, Lf, ldf, gp, s);
+  {
+    GemmArgs g{};
+    g.A = A; g.lda = p->n_pad; g.a_kmajor = 1;
+    g.B = A; g.ldb = p->n_pad; g.b_kmajor = 1;
+    g.C = Lf; g.ldc = ldf; g.M = m_pad; g.N = m_pad; g.K = p->n_pad;
+    g.alpha_neg = 1; g.beta_one = 1; g.lower_only = 1;
+    launch_gemm<T>(g, s);
+  }
+  launch_border_init<T>(Lf, ldf, M, m_pad, Yd, M, S, 2, 0.0, mu, s);  // border = (Y - mu)'
+  CK(sc.alloc(&tmp, (size_t)(nblk + TILE + 2) * sizeof(double)));
+  double* dscal = (double*)tmp;
+  CK(sc.alloc(&tmp, sizeof(int)));
+  int* dinfo = (int*)tmp;
+  CK(cudaMemsetAsync(dinfo, 0, sizeof(int), s));
+  prof_begin(ctx);
+  cholesky_inplace<T>(ctx, Lf, ldf, m_pad, ldf, Dinv, dscal, dinfo);
+  *Lf_out = Lf; *Dinv_out = Dinv; *dscal_out = dscal; *dinfo_out = dinfo;
+  return AGP_OK;
+}
+
+// waits for the stream and reports a failed factorisation of the posterior covariance
+inline int post_cov_status(agp_ctx* ctx, const int* dinfo) {
+  int h_info = 0;
+  CK(cudaMemcpyAsync(&h_info, dinfo, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  CK(cudaGetLastError());
+  if (h_info != 0) {
+    ctx->info = h_info;
+    char b[128];
+    snprintf(b, sizeof(b), "posterior covariance is not positive definite; Cholesky failed at pivot %d", h_info);
+    ctx->err = b;
+    return AGP_ERR_NOT_POSDEF;
+  }
+  return AGP_OK;
+}
+
 template <typename T>
 int post_cond_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp_mean* mean_s,
                    const agp_noise* noise_s, const void* Y, int S, void* logpdf_out, const void* Z, int Sz,
@@ -1104,18 +1174,15 @@ int post_cond_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp
   if (S < 0 || S > TILE) { ctx->err = "number of right-hand sides must be in [0,128]"; return AGP_ERR_UNSUPPORTED; }
   if (S > 0 && (!Y || !logpdf_out)) { ctx->err = "Y/logpdf_out is NULL"; return AGP_ERR_INVALID; }
   if (Sz > 0 && (!Z || !rand_out)) { ctx->err = "Z/out is NULL"; return AGP_ERR_INVALID; }
-  static const agp_noise default_noise{0, 1e-18, nullptr};  // default_sigma^2, finite_gp_projection.jl:17
-  if (!noise_s) noise_s = &default_noise;
-  if (noise_s->kind == 1 && !noise_s->v) { ctx->err = "noise vector is NULL"; return AGP_ERR_INVALID; }
-  agp_mean mz{p->mean_kind, p->mean_c, nullptr};
-  if (!mean_s) mean_s = &mz;
-  if (mean_s->kind == 2 && !mean_s->v) { ctx->err = "mean vector is NULL"; return AGP_ERR_INVALID; }
+  agp_mean mz;
+  int rc = post_side_defaults(p, &mean_s, &noise_s, &mz);
+  if (rc) return rc;
 
   const int64_t m_pad = round_up(M, TILE), ldf = m_pad + TILE;
   const int nblk = (int)(m_pad / TILE);
   Scratch sc(ctx);
   T *Xst = nullptr, *B = nullptr;
-  int rc = post_cross<T>(p, sc, layout, Xs, M, m_pad, &Xst, &B);
+  rc = post_cross<T>(p, sc, layout, Xs, M, m_pad, &Xst, &B);
   if (rc) return rc;
   T *mean_d = nullptr, *noise_d = nullptr, *Yd = nullptr;
   if (mean_s->kind == 2) { rc = upload<T>(ctx, sc, mean_s->v, M, true, &mean_d); if (rc) return rc; }
@@ -1128,48 +1195,20 @@ int post_cond_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp
   // posterior mean m* = m(x*) + K(x*, x) alpha, then V = L^-1 K(x, x*) in place
   launch_gemv_t<T>(B, p->n_pad, p->n_pad, M, (const T*)p->alpha, mean_s->kind, mean_s->c, mean_d, mu, s);
   forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, p->n_pad, B, p->n_pad, m_pad);
-  // C* + Sigma* = K(x*, x*) + Sigma* - V'V, lower triangle, identity padding
-  CK(sc.alloc(&tmp, (size_t)ldf * m_pad * sizeof(T)));
-  T* Lf = (T*)tmp;
-  CK(sc.alloc(&tmp, (size_t)nblk * TILE * TILE * sizeof(T)));
-  T* Dinv = (T*)tmp;
-  GramParams gp{};
-  fill_gram_params<T>(gp, &p->k, 1, 1, M, M, noise_s, noise_d, p->comp);
-  launch_gram<T>(Xst, Xst, m_pad, m_pad, p->D, Lf, ldf, gp, s);
-  {
-    GemmArgs g{};
-    g.A = B; g.lda = p->n_pad; g.a_kmajor = 1;
-    g.B = B; g.ldb = p->n_pad; g.b_kmajor = 1;
-    g.C = Lf; g.ldc = ldf; g.M = m_pad; g.N = m_pad; g.K = p->n_pad;
-    g.alpha_neg = 1; g.beta_one = 1; g.lower_only = 1;
-    launch_gemm<T>(g, s);
-  }
-  launch_border_init<T>(Lf, ldf, M, m_pad, Yd, M, S, 2, 0.0, (const T*)mu, s);  // border = (Y - m*)'
-  CK(sc.alloc(&tmp, (size_t)(nblk + TILE + 2) * sizeof(double)));
-  double* dscal = (double*)tmp;
-  CK(sc.alloc(&tmp, sizeof(int)));
-  int* dinfo = (int*)tmp;
-  CK(cudaMemsetAsync(dinfo, 0, sizeof(int), s));
+  T *Lf = nullptr, *Dinv = nullptr;
+  double* dscal = nullptr;
+  int* dinfo = nullptr;
+  rc = post_cov_factor<T>(p, sc, Xst, B, M, noise_s, noise_d, Yd, S, mu, &Lf, &Dinv, &dscal, &dinfo);
+  if (rc) return rc;
   CK(sc.alloc(&tmp, (size_t)TILE * sizeof(T)));
   T* lp_d = (T*)tmp;
-  prof_begin(ctx);
-  cholesky_inplace<T>(ctx, Lf, ldf, m_pad, ldf, Dinv, dscal, dinfo);
   if (S > 0) {
     CK(sc.alloc(&tmp, (size_t)S * m_pad * sizeof(T)));
     launch_extract_v<T>(Lf, ldf, m_pad, S, (T*)tmp, dscal + nblk, s);
     launch_finalize_logpdf<T>(dscal, nblk, dscal + nblk, S, M, lp_d, dscal + nblk + TILE, s);
   }
-  int h_info = 0;
-  CK(cudaMemcpyAsync(&h_info, dinfo, sizeof(int), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  if (h_info != 0) {
-    ctx->info = h_info;
-    char b[128];
-    snprintf(b, sizeof(b), "posterior covariance is not positive definite; Cholesky failed at pivot %d", h_info);
-    ctx->err = b;
-    return AGP_ERR_NOT_POSDEF;
-  }
+  rc = post_cov_status(ctx, dinfo);
+  if (rc) return rc;
   if (S > 0) CK(cudaMemcpyAsync(logpdf_out, lp_d, (size_t)S * sizeof(T), cudaMemcpyDeviceToHost, s));
   if (Sz > 0) {  // out = m* + L* Z  (C.U' * randn, finite_gp_projection.jl:235)
     const int64_t s_pad = round_up(Sz, 4);
@@ -1208,6 +1247,33 @@ static CompositeDesc single_kernel_desc(int family, double variance, double line
   one.acc_kind[0] = family == AGP_LINEAR ? COMP_ACC_DOT : COMP_ACC_SQ;
   one.w = nullptr;
   return one;
+}
+
+// the single-kernel slots of a gradient (agp.h's layout) from grad_reduce_kernel's sums h: [0] variance, [1] the Scale
+// factor, [2] LinearKernel c and [5..] the ARD values (ard_h, host copy of the transform's); slots 3 and 4 are the
+// caller's
+template <typename T>
+void single_kernel_grad(const agp_kernel& k, int D, const double* h, const T* ard_h, double* grad_out) {
+  const bool linear = k.family == AGP_LINEAR;
+  const bool want_ard = k.transform == AGP_T_ARD;
+  const double var = k.variance, sc_ = k.scale;
+  grad_out[0] = 0.5 * h[0];
+  grad_out[1] = (k.transform == AGP_T_SCALE) ? (linear ? var * h[1] / sc_ : 0.5 * var * h[1] / sc_) : 0.0;
+  grad_out[2] = linear ? 0.5 * var * h[2] : 0.0;
+  for (int d = 0; d < D; ++d)
+    grad_out[5 + d] = want_ard ? (linear ? var : 0.5 * var) * h[(size_t)5 + d] / (double)ard_h[(size_t)d] : 0.0;
+}
+
+// sum_i v_i of a device vector on the host, in index order and in double
+template <typename T>
+int host_sum(agp_ctx* ctx, const T* v, int64_t n, double* out) {
+  std::vector<T> h((size_t)n);
+  CK(cudaMemcpyAsync(h.data(), v, (size_t)n * sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  double c = 0.0;
+  for (int64_t i = 0; i < n; ++i) c += (double)h[(size_t)i];
+  *out = c;
+  return AGP_OK;
 }
 
 // The reductions that end every gradient of this form, on the handle's points and kernel: with W = alpha alpha' - Cinv
@@ -1281,15 +1347,9 @@ int grad_reductions_on(agp_post* p, Scratch& sc, const T* X, int64_t n, int64_t 
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
   if (!grad_out) return AGP_OK;
-  const bool linear = p->k.family == AGP_LINEAR;
-  const double var = p->k.variance, sc_ = p->k.scale;
-  grad_out[0] = 0.5 * h[0];
-  grad_out[1] = (p->k.transform == AGP_T_SCALE) ? (linear ? var * h[1] / sc_ : 0.5 * var * h[1] / sc_) : 0.0;
-  grad_out[2] = linear ? 0.5 * var * h[2] : 0.0;
+  single_kernel_grad<T>(p->k, D, h.data(), ard_h.data(), grad_out);
   grad_out[3] = 0.5 * h[3];
   grad_out[4] = h[4];
-  for (int d = 0; d < D; ++d)
-    grad_out[5 + d] = want_ard ? (linear ? var : 0.5 * var) * h[(size_t)5 + d] / (double)ard_h[(size_t)d] : 0.0;
   return AGP_OK;
 }
 
@@ -1301,12 +1361,17 @@ int grad_reductions(agp_post* p, Scratch& sc, const T* Cinv, const T* alpha, dou
 }
 
 
+inline int check_layout(agp_ctx* ctx, int layout) {
+  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
+  return AGP_OK;
+}
+
 // what every logpdf gradient of a handle checks first: the input layout, the factor gathered whole, a handle straight
 // from agp_fit
 template <typename T>
 int logpdf_grad_prelude(agp_post* p, int layout) {
   agp_ctx* ctx = p->ctx;
-  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
+  { int rc = check_layout(ctx, layout); if (rc) return rc; }
   { int rrc = post_replicate<T>(p); if (rrc) return rrc; }
   CK(cudaSetDevice(ctx->device));
   if (p->valid || p->segs.size() > 1) { ctx->err = "gradient of an extended (sequentially conditioned) posterior is unsupported"; return AGP_ERR_UNSUPPORTED; }
@@ -1351,13 +1416,73 @@ int post_logpdf_grad_impl(agp_post* p, double* grad_out, void* noise_diag_out, i
   return grad_reductions<T>(p, sc, Cinv, (const T*)p->alpha, grad_out, noise_diag_out, layout, x_grad_out);
 }
 
+// The column pullback of sum_s w_s logpdf(N(m, C), Y[:, s]) shared by the _cols and the held-out gradients.  C = L L' has
+// n rows (n_pad padded); L, lda, Dinv are its blocked factor and V = L^-1 (leading dimension n_pad).  The S columns of Y
+// (n x S, the caller's memory space) go through in chunks of up to 1024 with delta = Y - m (m: mean kind / c / device
+// vector), B_c = L^-1 delta_c, A_c = V' B_c = C^-1 delta_c and w = lp_bar (all ones when NULL):
+//   negW  = (sum w) C^-1 - sum_c A_c diag(w_c) A_c'   (negW holds C^-1 on entry; its lower tiles only with lower_only)
+//   mbar += A_c w_c,  y_bar_out = -A diag(w) (n x S, the caller's memory space),  sq_s += |L^-1 delta_s|^2.
+// Each output may be NULL.  w and the two n_pad x min(S, 1024) chunk buffers stay in sc.
+template <typename T>
+int weighted_cols_pullback(agp_ctx* ctx, Scratch& sc, const T* L, int64_t lda, const T* Dinv, int64_t n_pad, const T* V,
+                           int64_t n, const void* Y, int mean_kind, double mean_c, const T* mean_d, int S,
+                           const double* lp_bar, bool lower_only, T* negW, T* mbar, void* y_bar_out, T* sq) {
+  cudaStream_t s = ctx->stream;
+  std::vector<double> w((size_t)S, 1.0);
+  if (lp_bar) w.assign(lp_bar, lp_bar + S);
+  double wsum = 0.0;
+  for (double v : w) wsum += v;
+  std::vector<T> hw((size_t)2 * S);  // w, then -w
+  for (int j = 0; j < S; ++j) { hw[(size_t)j] = (T)w[(size_t)j]; hw[(size_t)S + j] = (T)-w[(size_t)j]; }
+  T* wd = nullptr;
+  int rc = upload<T>(ctx, sc, hw.data(), hw.size(), true, &wd);
+  if (rc) return rc;
+  const int64_t chunk = 1024, cmax = round_up(S < chunk ? S : chunk, TILE);
+  void* tmp = nullptr;
+  CK(sc.alloc(&tmp, (size_t)n_pad * cmax * sizeof(T) * 2));
+  T* B = (T*)tmp;  // delta_c, L^-1 delta_c, then Ybar_c
+  T* A = B + n_pad * cmax;
+  if (negW && wsum != 1.0) launch_scale<T>(negW, n_pad * n_pad, wsum, s);
+  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  for (int64_t c0 = 0; c0 < S; c0 += chunk) {
+    const int64_t nc = (S - c0 < chunk) ? (S - c0) : chunk, nc_pad = round_up(nc, TILE);
+    Scratch scc(ctx);
+    T* Yd = nullptr;
+    rc = upload<T>(ctx, scc, (const T*)Y + (size_t)c0 * n, (size_t)n * nc, false, &Yd);
+    if (rc) return rc;
+    launch_sub_mean_cols<T>(Yd, n, n, nc, mean_kind, mean_c, mean_d, B, n_pad, n_pad, nc_pad, s);
+    forward_subst_multi<T>(ctx, L, lda, Dinv, n_pad, B, n_pad, nc_pad);
+    if (sq) launch_colsumsq_acc<T>(B, n_pad, n, nc, 1.0, sq + c0, s);
+    {
+      GemmArgs g{};  // A_c = V' B_c
+      g.A = V; g.lda = n_pad; g.a_kmajor = 1;
+      g.B = B; g.ldb = n_pad; g.b_kmajor = 1;
+      g.C = A; g.ldc = n_pad; g.M = n_pad; g.N = nc_pad; g.K = n_pad;
+      launch_gemm<T>(g, s);
+    }
+    if (mbar) launch_gemv_n_acc<T>(A, n_pad, n, nc, wd + c0, mbar, s);
+    CK(cudaMemcpyAsync(B, A, (size_t)n_pad * nc_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    launch_scale_cols<T>(B, n_pad, n_pad, nc, wd + S + c0, s);  // Ybar_c = A_c diag(-w_c)
+    if (negW) {
+      GemmArgs g{};  // negW += Ybar_c A_c'
+      g.A = B; g.lda = n_pad; g.a_kmajor = 0;
+      g.B = A; g.ldb = n_pad; g.b_kmajor = 0;
+      g.C = negW; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = nc_pad; g.beta_one = 1; g.lower_only = lower_only ? 1 : 0;
+      launch_gemm<T>(g, s);
+    }
+    if (y_bar_out)
+      CK(cudaMemcpy2DAsync((T*)y_bar_out + (size_t)c0 * n, (size_t)n * sizeof(T), B, (size_t)n_pad * sizeof(T), (size_t)n * sizeof(T),
+                           (size_t)nc, kout, s));
+  }
+  return AGP_OK;
+}
+
 // ---- pullback of sum_s w_s logpdf(fx, Y[:, s]) on a handle from agp_fit (agp.h agp_post_logpdf_grad_cols).  With
 // delta_s = Y[:, s] - m, A = C^-1 [delta_1 .. delta_S] and w = lp_bar:
 //   -W = (sum_s w_s) C^-1 - A diag(w) A'   into the lower tiles of the C^-1 buffer,  mbar = A w,  Ybar = -A diag(w)
-// and then the reductions of agp_post_logpdf_grad_x with alpha = 0 and C^-1 replaced by -W.  The columns go through in
-// chunks of up to 1024 (fit_many_impl's): Delta_c = Y_c - m, B_c = L^-1 Delta_c, A_c = V' B_c on the tile GEMM (V = L^-1,
-// as C^-1 = V'V is formed: the same accuracy class), Ybar_c = A_c diag(-w_c), -W += Ybar_c A_c' (a rank-nc lower-only
-// GEMM), mbar += A_c w_c.  Two n_pad x n_pad and two n_pad x 1024 buffers of T whatever S is.
+// and then the reductions of agp_post_logpdf_grad_x with alpha = 0 and C^-1 replaced by -W.  The columns go through
+// weighted_cols_pullback in chunks of up to 1024 (fit_many_impl's), A_c = V' B_c on the tile GEMM (V = L^-1, as C^-1 =
+// V'V is formed: the same accuracy class).  Two n_pad x n_pad and two n_pad x 1024 buffers of T whatever S is.
 template <typename T>
 int post_logpdf_grad_cols_impl(agp_post* p, const agp_mean* mean, const void* Y, int S, const double* lp_bar,
                                double* grad_out, void* noise_diag_out, void* mean_diag_out, int layout, void* x_grad_out,
@@ -1375,58 +1500,17 @@ int post_logpdf_grad_cols_impl(agp_post* p, const agp_mean* mean, const void* Y,
   if (!mean) mean = &handle_mean;
   cudaStream_t s = ctx->stream;
   const int64_t N = p->n, n_pad = p->n_pad;
-  const int64_t chunk = 1024, cmax = round_up(S < chunk ? S : chunk, TILE);
   Scratch sc(ctx);
   T *V = nullptr, *Cinv = nullptr;  // Cinv becomes -W
   rc = inverse_factor<T>(p, sc, want_w, &V, &Cinv);
   if (rc) return rc;
   void* tmp = nullptr;
-  CK(sc.alloc(&tmp, (size_t)n_pad * cmax * sizeof(T) * 2));
-  T* B = (T*)tmp;  // Delta_c, L^-1 Delta_c, then Ybar_c
-  T* A = B + n_pad * cmax;
-  std::vector<double> w((size_t)S, 1.0);
-  if (lp_bar) w.assign(lp_bar, lp_bar + S);
-  double wsum = 0.0;
-  for (double v : w) wsum += v;
-  std::vector<T> hw((size_t)2 * S);  // w, then -w
-  for (int j = 0; j < S; ++j) { hw[(size_t)j] = (T)w[(size_t)j]; hw[(size_t)S + j] = (T)-w[(size_t)j]; }
-  T* wd = nullptr;
-  rc = upload<T>(ctx, sc, hw.data(), hw.size(), true, &wd);
-  if (rc) return rc;
   T *mbar = nullptr, *mean_d = nullptr;
   if (want_mbar) { CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T))); mbar = (T*)tmp; CK(cudaMemsetAsync(mbar, 0, (size_t)n_pad * sizeof(T), s)); }
   if (mean->kind == 2) { rc = upload<T>(ctx, sc, mean->v, N, true, &mean_d); if (rc) return rc; }
-  if (want_w && wsum != 1.0) launch_scale<T>(Cinv, n_pad * n_pad, wsum, s);
-  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
-  for (int64_t c0 = 0; c0 < S; c0 += chunk) {
-    const int64_t nc = (S - c0 < chunk) ? (S - c0) : chunk, nc_pad = round_up(nc, TILE);
-    Scratch scc(ctx);
-    T* Yd = nullptr;
-    rc = upload<T>(ctx, scc, (const T*)Y + (size_t)c0 * N, (size_t)N * nc, false, &Yd);
-    if (rc) return rc;
-    launch_sub_mean_cols<T>(Yd, N, N, nc, mean->kind, mean->c, mean_d, B, n_pad, n_pad, nc_pad, s);
-    forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, B, n_pad, nc_pad);
-    {
-      GemmArgs g{};  // A_c = V' B_c
-      g.A = V; g.lda = n_pad; g.a_kmajor = 1;
-      g.B = B; g.ldb = n_pad; g.b_kmajor = 1;
-      g.C = A; g.ldc = n_pad; g.M = n_pad; g.N = nc_pad; g.K = n_pad;
-      launch_gemm<T>(g, s);
-    }
-    if (want_mbar) launch_gemv_n_acc<T>(A, n_pad, N, nc, wd + c0, mbar, s);
-    CK(cudaMemcpyAsync(B, A, (size_t)n_pad * nc_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
-    launch_scale_cols<T>(B, n_pad, n_pad, nc, wd + S + c0, s);  // Ybar_c = A_c diag(-w_c)
-    if (want_w) {
-      GemmArgs g{};  // -W += Ybar_c A_c', lower tiles
-      g.A = B; g.lda = n_pad; g.a_kmajor = 0;
-      g.B = A; g.ldb = n_pad; g.b_kmajor = 0;
-      g.C = Cinv; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = nc_pad; g.beta_one = 1; g.lower_only = 1;
-      launch_gemm<T>(g, s);
-    }
-    if (y_bar_out)
-      CK(cudaMemcpy2DAsync((T*)y_bar_out + (size_t)c0 * N, (size_t)N * sizeof(T), B, (size_t)n_pad * sizeof(T), (size_t)N * sizeof(T),
-                           (size_t)nc, kout, s));
-  }
+  rc = weighted_cols_pullback<T>(ctx, sc, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, V, N, Y, mean->kind, mean->c,
+                                 mean_d, S, lp_bar, true, Cinv, mbar, y_bar_out, nullptr);
+  if (rc) return rc;
   if (want_w) {
     CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T)));
     T* zero_alpha = (T*)tmp;
@@ -1438,13 +1522,9 @@ int post_logpdf_grad_cols_impl(agp_post* p, const agp_mean* mean, const void* Y,
     rc = download<T>(ctx, mean_diag_out, mbar, (size_t)N, false);
     if (rc) return rc;
   }
-  if (grad_out) {  // d/d ConstMean c = sum_i mbar_i, in index order
-    std::vector<T> h((size_t)N);
-    CK(cudaMemcpyAsync(h.data(), mbar, (size_t)N * sizeof(T), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    double c = 0.0;
-    for (int64_t i = 0; i < N; ++i) c += (double)h[(size_t)i];
-    grad_out[4] = c;
+  if (grad_out) {  // d/d ConstMean c = sum_i mbar_i
+    rc = host_sum<T>(ctx, mbar, N, &grad_out[4]);
+    if (rc) return rc;
   }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
@@ -1482,13 +1562,10 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
   if (!Ys) { ctx->err = "Ys is NULL"; return AGP_ERR_INVALID; }
   if (!Xs) { ctx->err = "Xs is NULL"; return AGP_ERR_INVALID; }
   if (M <= 0) { ctx->err = "M must be positive"; return AGP_ERR_DIM_MISMATCH; }
-  static const agp_noise default_noise{0, 1e-18, nullptr};  // default_sigma^2, as agp_post_logpdf
-  if (!noise_s) noise_s = &default_noise;
-  if (noise_s->kind == 1 && !noise_s->v) { ctx->err = "noise vector is NULL"; return AGP_ERR_INVALID; }
-  agp_mean mz{p->mean_kind, p->mean_c, nullptr};
-  if (!mean_s) mean_s = &mz;
-  if (mean_s->kind == 2 && !mean_s->v) { ctx->err = "mean vector is NULL"; return AGP_ERR_INVALID; }
-  int rc = logpdf_grad_prelude<T>(p, layout);
+  agp_mean mz;
+  int rc = post_side_defaults(p, &mean_s, &noise_s, &mz);
+  if (rc) return rc;
+  rc = logpdf_grad_prelude<T>(p, layout);
   if (rc) return rc;
   cudaStream_t s = ctx->stream;
   const int64_t N = p->n, n_pad = p->n_pad, m_pad = round_up(M, TILE), ldf = m_pad + TILE;
@@ -1500,7 +1577,7 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
   Scratch sc(ctx);
   void* tmp = nullptr;
 
-  // ---- forward: mu*, A = L^-1 K_xs, Sigma = K_ss + Sigma* - A'A and its factor (post_cond_impl's)
+  // ---- forward: mu*, A = L^-1 K_xs, Sigma = K_ss + Sigma* - A'A and its factor
   T *Xst = nullptr, *A = nullptr;
   rc = post_cross<T>(p, sc, layout, Xs, M, m_pad, &Xst, &A);
   if (rc) return rc;
@@ -1512,44 +1589,16 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
   CK(cudaMemsetAsync(mu, 0, (size_t)m_pad * sizeof(T), s));
   launch_gemv_t<T>(A, n_pad, n_pad, M, (const T*)p->alpha, mean_s->kind, mean_s->c, mean_d, mu, s);
   forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, A, n_pad, m_pad);
-  CK(sc.alloc(&tmp, (size_t)ldf * m_pad * sizeof(T)));
-  T* Lf = (T*)tmp;
-  CK(sc.alloc(&tmp, (size_t)nblk * TILE * TILE * sizeof(T)));
-  T* Dinv = (T*)tmp;
-  {
-    GramParams gp{};
-    fill_gram_params<T>(gp, &p->k, 1, 1, M, M, noise_s, noise_d, p->comp);
-    launch_gram<T>(Xst, Xst, m_pad, m_pad, D, Lf, ldf, gp, s);
-    GemmArgs g{};
-    g.A = A; g.lda = n_pad; g.a_kmajor = 1;
-    g.B = A; g.ldb = n_pad; g.b_kmajor = 1;
-    g.C = Lf; g.ldc = ldf; g.M = m_pad; g.N = m_pad; g.K = n_pad;
-    g.alpha_neg = 1; g.beta_one = 1; g.lower_only = 1;
-    launch_gemm<T>(g, s);
-  }
-  launch_border_init<T>(Lf, ldf, M, m_pad, (const T*)nullptr, M, 0, 0, 0.0, (const T*)nullptr, s);
-  CK(sc.alloc(&tmp, (size_t)(nblk + TILE + 2) * sizeof(double)));
-  double* dscal = (double*)tmp;
-  CK(sc.alloc(&tmp, sizeof(int)));
-  int* dinfo = (int*)tmp;
-  CK(cudaMemsetAsync(dinfo, 0, sizeof(int), s));
-  prof_begin(ctx);
-  cholesky_inplace<T>(ctx, Lf, ldf, m_pad, ldf, Dinv, dscal, dinfo);
-  int h_info = 0;
-  std::vector<double> hld((size_t)nblk);
-  CK(cudaMemcpyAsync(&h_info, dinfo, sizeof(int), cudaMemcpyDeviceToHost, s));
-  CK(cudaMemcpyAsync(hld.data(), dscal, (size_t)nblk * sizeof(double), cudaMemcpyDeviceToHost, s));
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  if (h_info != 0) {
-    ctx->info = h_info;
-    char b[128];
-    snprintf(b, sizeof(b), "posterior covariance is not positive definite; Cholesky failed at pivot %d", h_info);
-    ctx->err = b;
-    return AGP_ERR_NOT_POSDEF;
-  }
+  T *Lf = nullptr, *Dinv = nullptr;
+  double* dscal = nullptr;
+  int* dinfo = nullptr;
+  rc = post_cov_factor<T>(p, sc, Xst, A, M, noise_s, noise_d, (const T*)nullptr, 0, mu, &Lf, &Dinv, &dscal, &dinfo);
+  if (rc) return rc;
+  rc = post_cov_status(ctx, dinfo);
+  if (rc) return rc;
   double logdet = 0.0;
-  for (double v : hld) logdet += v;
+  rc = host_sum<double>(ctx, dscal, nblk, &logdet);
+  if (rc) return rc;
   logdet *= 2.0;
 
   // ---- Sigma^-1 = Vs'Vs (Vs = L*^-1 with its identity padding zeroed, so nothing outside M x M is nonzero), then the
@@ -1563,60 +1612,19 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
   T* Ws = (T*)tmp;
   T* mubar = Ws + m_pad * m_pad;
   CK(cudaMemsetAsync(Ws, 0, (size_t)m_pad * (m_pad + XK) * sizeof(T), s));
-  std::vector<double> w((size_t)S, 1.0);
-  if (lp_bar) w.assign(lp_bar, lp_bar + S);
-  double wsum = 0.0;
-  for (double v : w) wsum += v;
   if (want_red) {
-    GemmArgs g{};  // (sum w) Sigma^-1, both triangles
+    GemmArgs g{};  // Sigma^-1, both triangles
     g.A = Vs; g.lda = m_pad; g.a_kmajor = 1;
     g.B = Vs; g.ldb = m_pad; g.b_kmajor = 1;
     g.C = Ws; g.ldc = m_pad; g.M = m_pad; g.N = m_pad; g.K = m_pad;
     launch_gemm<T>(g, s);
-    if (wsum != 1.0) launch_scale<T>(Ws, m_pad * m_pad, wsum, s);
   }
-  std::vector<T> hw((size_t)2 * S);  // w, then -w
-  for (int j = 0; j < S; ++j) { hw[(size_t)j] = (T)w[(size_t)j]; hw[(size_t)S + j] = (T)-w[(size_t)j]; }
-  T* wd = nullptr;
-  rc = upload<T>(ctx, sc, hw.data(), hw.size(), true, &wd);
-  if (rc) return rc;
   CK(sc.alloc(&tmp, (size_t)S * sizeof(T)));
   T* sq = (T*)tmp;
   CK(cudaMemsetAsync(sq, 0, (size_t)S * sizeof(T), s));
-  const int64_t chunk = 1024, cmax = round_up(S < chunk ? S : chunk, TILE);
-  CK(sc.alloc(&tmp, (size_t)m_pad * cmax * sizeof(T) * 2));
-  T* Bc = (T*)tmp;  // E_c, L*^-1 E_c, then Ybar*_c
-  T* Ac = Bc + m_pad * cmax;
-  for (int64_t c0 = 0; c0 < S; c0 += chunk) {
-    const int64_t nc = (S - c0 < chunk) ? (S - c0) : chunk, nc_pad = round_up(nc, TILE);
-    Scratch scc(ctx);
-    T* Yd = nullptr;
-    rc = upload<T>(ctx, scc, (const T*)Ys + (size_t)c0 * M, (size_t)M * nc, false, &Yd);
-    if (rc) return rc;
-    launch_sub_mean_cols<T>(Yd, M, M, nc, 2, 0.0, mu, Bc, m_pad, m_pad, nc_pad, s);
-    forward_subst_multi<T>(ctx, (const T*)Lf, ldf, (const T*)Dinv, m_pad, Bc, m_pad, nc_pad);
-    launch_colsumsq_acc<T>(Bc, m_pad, M, nc, 1.0, sq + c0, s);
-    {
-      GemmArgs g{};  // B_c = Vs' (L*^-1 E_c)
-      g.A = Vs; g.lda = m_pad; g.a_kmajor = 1;
-      g.B = Bc; g.ldb = m_pad; g.b_kmajor = 1;
-      g.C = Ac; g.ldc = m_pad; g.M = m_pad; g.N = nc_pad; g.K = m_pad;
-      launch_gemm<T>(g, s);
-    }
-    launch_gemv_n_acc<T>(Ac, m_pad, M, nc, wd + c0, mubar, s);
-    CK(cudaMemcpyAsync(Bc, Ac, (size_t)m_pad * nc_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
-    launch_scale_cols<T>(Bc, m_pad, m_pad, nc, wd + S + c0, s);  // Ybar*_c = B_c diag(-w_c)
-    if (want_red) {
-      GemmArgs g{};  // Ws += Ybar*_c B_c', both triangles
-      g.A = Bc; g.lda = m_pad; g.a_kmajor = 0;
-      g.B = Ac; g.ldb = m_pad; g.b_kmajor = 0;
-      g.C = Ws; g.ldc = m_pad; g.M = m_pad; g.N = m_pad; g.K = nc_pad; g.beta_one = 1;
-      launch_gemm<T>(g, s);
-    }
-    if (ys_bar_out)
-      CK(cudaMemcpy2DAsync((T*)ys_bar_out + (size_t)c0 * M, (size_t)M * sizeof(T), Bc, (size_t)m_pad * sizeof(T),
-                           (size_t)M * sizeof(T), (size_t)nc, kout, s));
-  }
+  rc = weighted_cols_pullback<T>(ctx, sc, (const T*)Lf, ldf, (const T*)Dinv, m_pad, Vs, M, Ys, 2, 0.0, mu, S, lp_bar,
+                                 false, want_red ? Ws : nullptr, mubar, ys_bar_out, sq);
+  if (rc) return rc;
   if (lp_out) {  // logpdf_s = -1/2 (M log 2 pi + logdet Sigma + |L*^-1 e_s|^2)
     std::vector<T> h((size_t)S);
     CK(cudaMemcpyAsync(h.data(), sq, (size_t)S * sizeof(T), cudaMemcpyDeviceToHost, s));
@@ -1718,15 +1726,11 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
       if (rc) return rc;
       rc = split_x(xs_grad_out, n_pad, M);
       if (rc) return rc;
-      if (grad_out) {  // d/d sigma^2 = sum_i Cbar_ii and d/d ConstMean c = sum mubar - sum beta, in index order
-        std::vector<T> hn((size_t)N), hb((size_t)N), hm((size_t)M);
-        CK(cudaMemcpyAsync(hn.data(), nd, (size_t)N * sizeof(T), cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(hb.data(), beta, (size_t)N * sizeof(T), cudaMemcpyDeviceToHost, s));
-        CK(cudaMemcpyAsync(hm.data(), mubar, (size_t)M * sizeof(T), cudaMemcpyDeviceToHost, s));
-        CK(cudaStreamSynchronize(s));
+      if (grad_out) {  // d/d sigma^2 = sum_i Cbar_ii and d/d ConstMean c = sum mubar - sum beta
         double sn = 0.0, sm = 0.0, sb = 0.0;
-        for (int64_t i = 0; i < N; ++i) { sn += (double)hn[(size_t)i]; sb += (double)hb[(size_t)i]; }
-        for (int64_t i = 0; i < M; ++i) sm += (double)hm[(size_t)i];
+        rc = host_sum<T>(ctx, nd, N, &sn); if (rc) return rc;
+        rc = host_sum<T>(ctx, beta, N, &sb); if (rc) return rc;
+        rc = host_sum<T>(ctx, mubar, M, &sm); if (rc) return rc;
         grad_out[3] = sn;
         grad_out[4] = sm - sb;
       }
@@ -2002,13 +2006,14 @@ int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
   const int64_t n_pad = p->n_pad, s_pad = round_up(S, 4);
   Scratch sc(ctx);
   void* tmp = nullptr;
-  // the three N x N buffers first (fit_impl's note on the stream-ordered pool)
+  const bool want_c = grad_out || noise_diag_out || x_grad_out;
+  // the three N x N buffers first (fit_impl's note on the stream-ordered pool); V only when the reductions run
   CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
   T* B1 = (T*)tmp;  // L', then W1 = Q V
   CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
   T* B2 = (T*)tmp;  // Q, then -V'QV (lower tiles)
-  CK(sc.alloc(&tmp, (size_t)n_pad * n_pad * sizeof(T)));
-  T* V = (T*)tmp;
+  T *V = nullptr, *unused = nullptr;
+  if (want_c) { rc = inverse_factor<T>(p, sc, false, &V, &unused); if (rc) return rc; }
   CK(sc.alloc(&tmp, (size_t)n_pad * s_pad * sizeof(T) * 3));
   T* Od = (T*)tmp; T* Zd = Od + n_pad * s_pad; T* Zb = Zd + n_pad * s_pad;
   CK(sc.alloc(&tmp, (size_t)n_pad * sizeof(T)));
@@ -2036,7 +2041,6 @@ int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
   }
   if (z_bar_out && S > 0)
     CK(cudaMemcpy2DAsync(z_bar_out, (size_t)N * sizeof(T), Zb, (size_t)n_pad * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kout, s));
-  const bool want_c = grad_out || noise_diag_out || x_grad_out;
   if (want_c) {
     {
       GemmArgs g{};  // Q = Zbar Z', lower tiles (K = S), then mirrored
@@ -2046,9 +2050,6 @@ int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
       launch_gemm<T>(g, s);
       launch_symmetrize_lower<T>(B2, n_pad, n_pad, s);
     }
-    CK(cudaMemsetAsync(V, 0, (size_t)n_pad * n_pad * sizeof(T), s));
-    launch_add_diag<T>(V, n_pad, n_pad, 1.0, s);
-    forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, V, n_pad, n_pad);
     {
       GemmArgs g{};  // W1 = Q V
       g.A = B2; g.lda = n_pad; g.a_kmajor = 0;
@@ -2068,13 +2069,9 @@ int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
   }
   rc = download<T>(ctx, mean_diag_out, mbar, (size_t)N, false);
   if (rc) return rc;
-  if (grad_out) {  // d/d ConstMean c = sum_i mbar_i, in index order
-    std::vector<double> h((size_t)N);
-    CK(cudaMemcpyAsync(h.data(), mbar, (size_t)N * sizeof(double), cudaMemcpyDeviceToHost, s));
-    CK(cudaStreamSynchronize(s));
-    double c = 0.0;
-    for (int64_t i = 0; i < N; ++i) c += h[(size_t)i];
-    grad_out[4] = c;
+  if (grad_out) {  // d/d ConstMean c = sum_i mbar_i
+    rc = host_sum<double>(ctx, mbar, N, &grad_out[4]);
+    if (rc) return rc;
   }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
@@ -2082,7 +2079,8 @@ int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
 }
 
 int rand_grad_check(agp_ctx* ctx, int layout, const void* X, const void* Z, int S, const void* out_bar) {
-  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
+  int rc = check_layout(ctx, layout);
+  if (rc) return rc;
   if (!X) { ctx->err = "X is NULL"; return AGP_ERR_INVALID; }
   if (S < 0) { ctx->err = "S must be >= 0"; return AGP_ERR_INVALID; }
   if (S > 0 && (!Z || !out_bar)) { ctx->err = "Z/out_bar is NULL"; return AGP_ERR_INVALID; }
@@ -2090,87 +2088,131 @@ int rand_grad_check(agp_ctx* ctx, int layout, const void* X, const void* Z, int 
   return AGP_OK;
 }
 
+// An fp32 problem converted to fp64, for the gradients whose pullback runs in fp64 (rand_grad_f32, vfe_grad_f32).
+// Parameter arrays are host memory (agp.h) and are widened on the host: the kernel's (the ARD values, or a composite's
+// factors' ard and r), the mean and noise vectors (n points) and the jitter vector (m inducing points).  Point sets,
+// targets and normals keep the caller's memory space: widened on the host, or cast into one fp64 scratch block on the
+// device.  The fp64 outputs likewise, and narrow() rounds them into the caller's fp32 outputs.  Everything the converted
+// problem points at lives as long as the object.
+struct Fp64Problem {
+  agp_ctx* ctx;
+  bool dev;
+  Scratch sc;
+  std::vector<std::vector<double>> keep;  // widened host arrays
+  agp_kernel k64{};
+  agp_kernel_composite c64{};
+  std::vector<agp_kernel_factor> f64;
+  agp_mean m64{};
+  agp_noise n64{}, j64{};
+  const agp_mean* mean = nullptr;  // the converted parameters, NULL where the caller's are
+  const agp_noise *noise = nullptr, *jitter = nullptr;
+  struct Out { const double* src; void* dst; int64_t n; };
+  std::vector<Out> outs;
+
+  explicit Fp64Problem(agp_ctx* c) : ctx(c), dev(c->memspace == AGP_MEM_DEVICE), sc(c) {}
+
+  const double* widen(const void* v, int64_t n) {
+    if (!v) return nullptr;
+    keep.emplace_back((size_t)n);
+    for (int64_t i = 0; i < n; ++i) keep.back()[(size_t)i] = (double)((const float*)v)[i];
+    return keep.back().data();
+  }
+
+  const agp_kernel* params(const agp_kernel* k, int D, const agp_mean* m_in, const agp_noise* n_in, int64_t n,
+                          const agp_noise* j_in, int64_t m) {
+    k64 = *k;
+    if (k->family == AGP_COMPOSITE && k->composite) {
+      c64 = *k->composite;
+      int nf = 0;
+      if (c64.nfactors && c64.nterms > 0 && c64.nterms <= AGP_COMP_MAX)
+        for (int t = 0; t < c64.nterms; ++t) nf += c64.nfactors[t] > 0 ? c64.nfactors[t] : 0;
+      if (c64.factors && nf <= AGP_COMP_MAX) {  // out-of-range descriptors are reported by comp_build
+        f64.assign(c64.factors, c64.factors + nf);
+        for (auto& f : f64) { f.ard = widen(f.ard, D); f.r = widen(f.r, D); }
+        c64.factors = f64.data();
+      }
+      k64.composite = &c64;
+    } else if (k->transform == AGP_T_ARD) {
+      k64.ard = widen(k->ard, D);
+    }
+    if (m_in) { m64 = *m_in; if (m_in->kind == 2) m64.v = widen(m_in->v, n); mean = &m64; }
+    if (n_in) { n64 = *n_in; if (n_in->kind == 1) n64.v = widen(n_in->v, n); noise = &n64; }
+    if (j_in) { j64 = *j_in; if (j_in->kind == 1) j64.v = widen(j_in->v, m); jitter = &j64; }
+    return &k64;
+  }
+
+  // fp64 copies of the fp32 arrays in (pointer, count); a NULL array stays NULL
+  int inputs(std::initializer_list<std::pair<const void*, int64_t>> in, const double** out) {
+    if (!dev) {
+      for (const auto& a : in) *out++ = widen(a.first, a.second);
+      return AGP_OK;
+    }
+    int64_t total = 0;
+    for (const auto& a : in) total += a.second;
+    void* tmp = nullptr;
+    CK(sc.alloc(&tmp, (size_t)total * sizeof(double)));
+    double* b = (double*)tmp;
+    for (const auto& a : in) {
+      *out = nullptr;
+      if (a.first) { launch_cast<float, double>((const float*)a.first, b, a.second, ctx->stream); *out = b; }
+      ++out;
+      b += a.second;
+    }
+    return AGP_OK;
+  }
+
+  // fp64 buffers for the fp32 outputs in (pointer, count); NULL where the output is not asked for
+  int outputs(std::initializer_list<std::pair<void*, int64_t>> o, double** out) {
+    int64_t total = 0;
+    for (const auto& a : o) if (a.first) total += a.second;
+    double* b = nullptr;
+    if (dev) { void* tmp = nullptr; CK(sc.alloc(&tmp, (size_t)total * sizeof(double))); b = (double*)tmp; }
+    for (const auto& a : o) {
+      *out = nullptr;
+      if (a.first) {
+        if (dev) { *out = b; b += a.second; }
+        else { keep.emplace_back((size_t)a.second); *out = keep.back().data(); }
+        outs.push_back(Out{*out, a.first, a.second});
+      }
+      ++out;
+    }
+    return AGP_OK;
+  }
+
+  int narrow() {
+    for (const Out& o : outs) {
+      if (o.n <= 0) continue;
+      if (!dev) { for (int64_t i = 0; i < o.n; ++i) ((float*)o.dst)[i] = (float)o.src[i]; }
+      else launch_cast<double, float>(o.src, (float*)o.dst, o.n, ctx->stream);
+    }
+    CK(cudaStreamSynchronize(ctx->stream));
+    CK(cudaGetLastError());
+    return AGP_OK;
+  }
+};
+
 // fp32 problems: the pullback is formed on the problem converted to fp64 and its outputs rounded to fp32.  -V'QV carries
-// terms of the order of cond(C) that cancel (agp.h).  Parameter arrays are host memory (widened here); X, Z, out_bar and
-// the array outputs keep the caller's memory space.
+// terms of the order of cond(C) that cancel (agp.h).
 int rand_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout, const void* X,
                   int64_t N, int D, const void* Z, int S, const void* out_bar, double* grad_out, void* noise_diag_out,
                   void* mean_diag_out, void* x_grad_out, void* z_bar_out) {
   int rc = check_kernel(ctx, k, D);
   if (rc) return rc;
   if (N <= 0) { ctx->err = "N must be positive"; return AGP_ERR_DIM_MISMATCH; }
-  cudaStream_t s = ctx->stream;
   CK(cudaSetDevice(ctx->device));
-  const bool dev = ctx->memspace == AGP_MEM_DEVICE;
-  std::vector<std::vector<double>> keep;  // widened host arrays, alive for the call
-  auto widen = [&](const void* v, int64_t n) -> const double* {
-    if (!v) return nullptr;
-    keep.emplace_back((size_t)n);
-    for (int64_t i = 0; i < n; ++i) keep.back()[(size_t)i] = (double)((const float*)v)[i];
-    return keep.back().data();
-  };
-  agp_kernel k64 = *k;
-  agp_kernel_composite c64{};
-  std::vector<agp_kernel_factor> f64;
-  if (k->family == AGP_COMPOSITE && k->composite) {
-    c64 = *k->composite;
-    int nf = 0;
-    if (c64.nfactors && c64.nterms > 0 && c64.nterms <= AGP_COMP_MAX)
-      for (int t = 0; t < c64.nterms; ++t) nf += c64.nfactors[t] > 0 ? c64.nfactors[t] : 0;
-    if (c64.factors && nf <= AGP_COMP_MAX) {  // out-of-range descriptors are reported by comp_build
-      f64.assign(c64.factors, c64.factors + nf);
-      for (auto& f : f64) { f.ard = widen(f.ard, D); f.r = widen(f.r, D); }
-      c64.factors = f64.data();
-    }
-    k64.composite = &c64;
-  } else if (k->transform == AGP_T_ARD) {
-    k64.ard = widen(k->ard, D);
-  }
-  agp_mean m64{};
-  agp_noise n64{};
-  if (mean) { m64 = *mean; if (mean->kind == 2) m64.v = widen(mean->v, N); }
-  if (noise) { n64 = *noise; if (noise->kind == 1) n64.v = widen(noise->v, N); }
-  Scratch sc(ctx);
-  const double *X64 = nullptr, *Z64 = nullptr, *O64 = nullptr;
-  double *nd64 = nullptr, *md64 = nullptr, *x64 = nullptr, *zb64 = nullptr;
-  std::vector<double> hnd, hmd, hx, hzb;
+  Fp64Problem p(ctx);
+  const agp_kernel* k64 = p.params(k, D, mean, noise, N, nullptr, 0);
   const int64_t NS = N * (int64_t)S;
-  if (!dev) {
-    X64 = widen(X, N * D); Z64 = widen(Z, NS); O64 = widen(out_bar, NS);
-    if (noise_diag_out) { hnd.resize((size_t)N); nd64 = hnd.data(); }
-    if (mean_diag_out) { hmd.resize((size_t)N); md64 = hmd.data(); }
-    if (x_grad_out) { hx.resize((size_t)(N * D)); x64 = hx.data(); }
-    if (z_bar_out) { hzb.resize((size_t)NS); zb64 = hzb.data(); }
-  } else {
-    void* tmp = nullptr;
-    CK(sc.alloc(&tmp, (size_t)(N * D + 2 * NS) * sizeof(double)));
-    double* b = (double*)tmp;
-    launch_cast<float, double>((const float*)X, b, N * D, s);
-    X64 = b;
-    if (Z) { launch_cast<float, double>((const float*)Z, b + N * D, NS, s); Z64 = b + N * D; }
-    if (out_bar) { launch_cast<float, double>((const float*)out_bar, b + N * D + NS, NS, s); O64 = b + N * D + NS; }
-    CK(sc.alloc(&tmp, (size_t)(2 * N + N * D + NS) * sizeof(double)));
-    double* o = (double*)tmp;
-    if (noise_diag_out) nd64 = o;
-    if (mean_diag_out) md64 = o + N;
-    if (x_grad_out) x64 = o + 2 * N;
-    if (z_bar_out) zb64 = o + 2 * N + N * D;
-  }
-  rc = rand_grad_f64(ctx, &k64, mean ? &m64 : nullptr, noise ? &n64 : nullptr, layout, X64, N, D, Z64, S, O64, grad_out, nd64,
-                     md64, x64, zb64);
+  const double* in[3];  // X, Z, out_bar
+  rc = p.inputs({{X, N * D}, {Z, NS}, {out_bar, NS}}, in);
   if (rc) return rc;
-  auto narrow = [&](const double* src, void* dst, int64_t n) {
-    if (!dst || n <= 0) return;
-    if (!dev) { for (int64_t i = 0; i < n; ++i) ((float*)dst)[i] = (float)src[i]; return; }
-    launch_cast<double, float>(src, (float*)dst, n, s);
-  };
-  narrow(nd64, noise_diag_out, N);
-  narrow(md64, mean_diag_out, N);
-  narrow(x64, x_grad_out, N * D);
-  narrow(zb64, z_bar_out, NS);
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  return AGP_OK;
+  double* out[4];  // noise_diag, mean_diag, x_grad, z_bar
+  rc = p.outputs({{noise_diag_out, N}, {mean_diag_out, N}, {x_grad_out, N * D}, {z_bar_out, NS}}, out);
+  if (rc) return rc;
+  rc = rand_grad_f64(ctx, k64, p.mean, p.noise, layout, in[0], N, D, in[1], S, in[2], grad_out, out[0], out[1],
+                     out[2], out[3]);
+  if (rc) return rc;
+  return p.narrow();
 }
 
 template <typename T>
@@ -2413,6 +2455,16 @@ int vfe_core(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
 }
 
 // ---- gradient of the VFE objectives (agp_vfe_elbo_grad; the formulas are in agp.h and vfe_grad.cu) ----------------
+int vfe_grad_check(agp_ctx* ctx, const agp_kernel* k, int layout, int objective) {
+  if (objective != 0 && objective != 1) { ctx->err = "objective must be 0 (elbo) or 1 (DTC)"; return AGP_ERR_INVALID; }
+  int rc = check_layout(ctx, layout);
+  if (rc) return rc;
+  if (k && k->family == AGP_COMPOSITE) { ctx->err = "composite kernels are supported on the exact path only (not VFE)"; return AGP_ERR_UNSUPPORTED; }
+  if (ctx->nccl) { ctx->err = "the VFE gradient runs on a single-GPU context"; return AGP_ERR_UNSUPPORTED; }
+  return AGP_OK;
+}
+
+
 // Pass 1 is vfe_core's.  Then, once: V_z = L_z^-1 and V_m = L_m^-1 by the forward substitution on the identity,
 // Lam^-1 = V_m' V_m, H and E, R = V_z' H V_z, P = V_z' E V_z = -2 Kbar_zz and r = V_z' m_e (O(M^3), tile GEMMs).  The K_zz
 // part goes through the exact path's reductions with alpha = 0 and C^-1 = P: grad_reduce_kernel gives
@@ -2424,10 +2476,6 @@ int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
                   const void* X, int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y,
                   int objective, void* value_out, double* grad_out, void* noise_diag_out, void* mean_diag_out,
                   void* z_grad_out, void* x_grad_out) {
-  if (objective != 0 && objective != 1) { ctx->err = "objective must be 0 (elbo) or 1 (DTC)"; return AGP_ERR_INVALID; }
-  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
-  if (k && k->family == AGP_COMPOSITE) { ctx->err = "composite kernels are supported on the exact path only (not VFE)"; return AGP_ERR_UNSUPPORTED; }
-  if (ctx->nccl) { ctx->err = "the VFE gradient runs on a single-GPU context"; return AGP_ERR_UNSUPPORTED; }
   const double c = objective == 0 ? 1.0 : 0.0;
   const VfeAfter<T> grad = [&](const VfePass<T>& p) -> int {
     cudaStream_t s = ctx->stream;
@@ -2555,14 +2603,9 @@ int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
     CK(cudaGetLastError());
     if (value_out) { const T v = (T)(objective == 0 ? p.elbo : p.dtc); memcpy(value_out, &v, sizeof(T)); }
     if (!grad_out) return AGP_OK;
-    const double var = k->variance, sc_ = k->scale;  // the mapping of post_logpdf_grad_impl
-    grad_out[0] = 0.5 * h[0];
-    grad_out[1] = (k->transform == AGP_T_SCALE) ? (linear ? var * h[1] / sc_ : 0.5 * var * h[1] / sc_) : 0.0;
-    grad_out[2] = linear ? 0.5 * var * h[2] : 0.0;
+    single_kernel_grad<T>(*k, D, h.data(), ard_h.data(), grad_out);
     grad_out[3] = h[(size_t)nsums];
     grad_out[4] = h[(size_t)nsums + 1];
-    for (int d = 0; d < D; ++d)
-      grad_out[5 + d] = want_ard ? (linear ? var : 0.5 * var) * h[(size_t)5 + d] / (double)ard_h[(size_t)d] : 0.0;
     return AGP_OK;
   };
   return vfe_core<T>(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, nullptr, nullptr, nullptr, &grad);
@@ -2575,10 +2618,6 @@ int vfe_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const 
                  int64_t N, int D, const void* Zind, int64_t M, const agp_noise* jitter, const void* y, int objective,
                  void* value_out, double* grad_out, void* noise_diag_out, void* mean_diag_out, void* z_grad_out,
                  void* x_grad_out) {
-  if (objective != 0 && objective != 1) { ctx->err = "objective must be 0 (elbo) or 1 (DTC)"; return AGP_ERR_INVALID; }
-  if (layout != AGP_POINT_MAJOR && layout != AGP_FEATURE_MAJOR) { ctx->err = "layout must be AGP_POINT_MAJOR or AGP_FEATURE_MAJOR"; return AGP_ERR_INVALID; }
-  if (k && k->family == AGP_COMPOSITE) { ctx->err = "composite kernels are supported on the exact path only (not VFE)"; return AGP_ERR_UNSUPPORTED; }
-  if (ctx->nccl) { ctx->err = "the VFE gradient runs on a single-GPU context"; return AGP_ERR_UNSUPPORTED; }
   int rc = check_kernel(ctx, k, D);
   if (rc) return rc;
   if (N <= 0 || M <= 0) { ctx->err = "N and M must be positive"; return AGP_ERR_DIM_MISMATCH; }
@@ -2589,67 +2628,18 @@ int vfe_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const 
     if (rc) return rc;
     memcpy(value_out, &v[objective], sizeof(float));
   }
-  cudaStream_t s = ctx->stream;
-  const bool dev = ctx->memspace == AGP_MEM_DEVICE;
-  auto widen = [](const void* v, int64_t n) {  // host-side parameter arrays (always host memory, agp.h)
-    std::vector<double> out((size_t)n);
-    for (int64_t i = 0; i < n; ++i) out[(size_t)i] = (double)((const float*)v)[i];
-    return out;
-  };
-  agp_kernel k64 = *k;
-  std::vector<double> ard64, mean64, noise64, jit64;
-  if (k->transform == AGP_T_ARD && k->ard) { ard64 = widen(k->ard, D); k64.ard = ard64.data(); }
-  agp_mean m64{};
-  agp_noise n64{}, j64{};
-  if (mean) { m64 = *mean; if (mean->kind == 2 && mean->v) { mean64 = widen(mean->v, N); m64.v = mean64.data(); } }
-  if (noise) { n64 = *noise; if (noise->kind == 1 && noise->v) { noise64 = widen(noise->v, N); n64.v = noise64.data(); } }
-  if (jitter) { j64 = *jitter; if (jitter->kind == 1 && jitter->v) { jit64 = widen(jitter->v, M); j64.v = jit64.data(); } }
-  // the point sets, the targets and the outputs: host vectors, or device buffers under AGP_MEM_DEVICE
-  Scratch sc(ctx);
-  std::vector<double> hX, hZ, hy, hnd, hmd, hz, hx;
-  const void *X64, *Z64, *y64;
-  double *nd64 = nullptr, *md64 = nullptr, *z64 = nullptr, *x64 = nullptr;
-  if (!dev) {
-    hX = widen(X, N * D); hZ = widen(Zind, M * D); hy = widen(y, N);
-    X64 = hX.data(); Z64 = hZ.data(); y64 = hy.data();
-    if (noise_diag_out) { hnd.resize((size_t)N); nd64 = hnd.data(); }
-    if (mean_diag_out) { hmd.resize((size_t)N); md64 = hmd.data(); }
-    if (z_grad_out) { hz.resize((size_t)(M * D)); z64 = hz.data(); }
-    if (x_grad_out) { hx.resize((size_t)(N * D)); x64 = hx.data(); }
-  } else {
-    void* tmp = nullptr;
-    CK(sc.alloc(&tmp, (size_t)(N * D + M * D + N) * sizeof(double)));
-    double* b = (double*)tmp;
-    launch_cast<float, double>((const float*)X, b, N * D, s);
-    launch_cast<float, double>((const float*)Zind, b + N * D, M * D, s);
-    launch_cast<float, double>((const float*)y, b + N * D + M * D, N, s);
-    X64 = b; Z64 = b + N * D; y64 = b + N * D + M * D;
-    CK(sc.alloc(&tmp, (size_t)(2 * N + M * D) * sizeof(double)));
-    double* o = (double*)tmp;
-    if (noise_diag_out) nd64 = o;
-    if (mean_diag_out) md64 = o + N;
-    if (z_grad_out) z64 = o + 2 * N;
-    if (x_grad_out) { CK(sc.alloc(&tmp, (size_t)N * D * sizeof(double))); x64 = (double*)tmp; }
-  }
-  rc = vfe_grad_impl<double>(ctx, &k64, mean ? &m64 : nullptr, noise ? &n64 : nullptr, layout, X64, N, D, Z64, M,
-                             jitter ? &j64 : nullptr, y64, objective, nullptr, grad_out, nd64, md64, z64, x64);
+  Fp64Problem p(ctx);
+  const agp_kernel* k64 = p.params(k, D, mean, noise, N, jitter, M);
+  const double* in[3];  // X, Z, y
+  rc = p.inputs({{X, N * D}, {Zind, M * D}, {y, N}}, in);
   if (rc) return rc;
-  auto narrow = [&](const double* src, void* dst, int64_t n) -> int {
-    if (!dst) return AGP_OK;
-    if (!dev) {
-      for (int64_t i = 0; i < n; ++i) ((float*)dst)[i] = (float)src[i];
-      return AGP_OK;
-    }
-    launch_cast<double, float>(src, (float*)dst, n, s);
-    return AGP_OK;
-  };
-  narrow(nd64, noise_diag_out, N);
-  narrow(md64, mean_diag_out, N);
-  narrow(z64, z_grad_out, M * D);
-  narrow(x64, x_grad_out, N * D);
-  CK(cudaStreamSynchronize(s));
-  CK(cudaGetLastError());
-  return AGP_OK;
+  double* out[4];  // noise_diag, mean_diag, z_grad, x_grad
+  rc = p.outputs({{noise_diag_out, N}, {mean_diag_out, N}, {z_grad_out, M * D}, {x_grad_out, N * D}}, out);
+  if (rc) return rc;
+  rc = vfe_grad_impl<double>(ctx, k64, p.mean, p.noise, layout, in[0], N, D, in[1], M, p.jitter, in[2],
+                             objective, nullptr, grad_out, out[0], out[1], out[2], out[3]);
+  if (rc) return rc;
+  return p.narrow();
 }
 
 template <typename T>
@@ -3605,6 +3595,8 @@ int32_t agp_vfe_elbo_grad_x(agp_ctx* ctx, int32_t dtype, const agp_kernel* k, co
                             const agp_noise* jitter, const void* y, int32_t objective, void* value_out, double* grad_out,
                             void* noise_diag_out, void* mean_diag_out, void* z_grad_out, void* x_grad_out) {
   if (!ctx) return AGP_ERR_INVALID;
+  int rc = vfe_grad_check(ctx, k, layout, objective);
+  if (rc) return rc;
   return DISPATCH(dtype,
                   vfe_grad_f32(ctx, k, mean, noise, layout, X, N, D, Zind, M, jitter, y, objective, value_out, grad_out,
                                noise_diag_out, mean_diag_out, z_grad_out, x_grad_out),
