@@ -82,6 +82,8 @@ SIGNATURES = {
                                               C.c_int32, _P, _P]),
     "agp_post_pred_logpdf_grad": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _M, _N, _P, C.c_int32, C.POINTER(C.c_double), _P,
                                               C.POINTER(C.c_double), _P, _P, _P, _P, _P, _P, _P, _P]),
+    "agp_post_rand_grad": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _M, _N, _P, C.c_int32, _P, C.POINTER(C.c_double), _P,
+                                       _P, _P, _P, _P, _P, _P, _P]),
     "agp_post_grad_len": (C.c_int64, [_P]),
     "agp_post_solve_lower": (C.c_int32, [_P, _P, C.c_int64, _P]),
     "agp_post_factor_export": (C.c_int32, [_P, _P]),

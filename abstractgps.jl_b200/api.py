@@ -1070,6 +1070,57 @@ def posterior_logpdf_grad(fx: FiniteGP, Y, lp_bar=None, inputs=False):
     return (lp[0] if ndim == 1 else lp), res
 
 
+def posterior_rand_grad(fx: FiniteGP, Z, out_bar, inputs=False):
+    """(out, gradient dict) of the posterior samples out = rand(fx, S) = mu* + L* Z at the caller's standard normals Z,
+    pulled back from the cotangent out_bar, for fx = p(x*, s2*) over an exact posterior p = posterior(fx0, y): what
+    Zygote returns through rand over a posterior, for Monte Carlo acquisition functions and losses built on
+    reparameterised samples.  One agp_post_rand_grad call on p's handle; out is agp_post_rand's at the same Z.  Z and
+    out_bar are M x S (or vectors as one column).  The dict has the keys of posterior_logpdf_grad with "Z" (the cotangent
+    of the normals, shaped like Z) in place of "Y": the kernel keys, the training side "noise", "mean_c" | "mean_v" and
+    "y", the test side "noise_s" and "mean_s_v"; a ConstMean's "mean_c" counts both sides.  inputs=True also returns
+    "x" and "xs", shaped like the containers the points came in.  A CustomMean is treated as a constant of the inputs.
+    Only a posterior straight from posterior(fx0, y) is supported (not a sequentially conditioned one)."""
+    p = fx.f
+    if not isinstance(p, PosteriorGP) or getattr(p, "fx", None) is None:
+        raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "the gradient of rand over a posterior needs a FiniteGP over "
+                       "posterior(fx, y), not over %s" % type(p).__name__)
+    eng = engine()
+    p, dt, pts, ms, ns, keep = _post_args(fx)
+    fx0 = p.fx
+    N, M, D = p.data.x.n, pts.n, pts.D
+    ndim, Zf, S, _ = _cols_and_weights(Z, None, M, dt)
+    _, Ob, _, _ = _cols_and_weights(out_bar, None, M, dt)
+    if Ob.shape != Zf.shape:
+        raise DimensionMismatch("out_bar has shape %s, Z has %s" % (Ob.shape, Zf.shape))
+    f = p.prior
+    k = f.kernel
+    g, flat = _grad_buffer(k, D, p.data.C.h)
+    out = np.empty((M, S), dtype=dt, order="F")
+    eng.check(eng.L.agp_post_rand(p.data.C.h, cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), M, C.byref(ms), C.byref(ns),
+                                  cabi.ptr(Zf), S, cabi.ptr(out)))
+    nd = np.empty(N, dtype=dt) if np.ndim(fx0.s2) != 0 else None
+    md = np.empty(N, dtype=dt) if isinstance(f.mean, CustomMean) else None
+    yb = np.empty(N, dtype=dt)
+    nsd = np.empty(M, dtype=dt)
+    msd = np.empty(M, dtype=dt) if isinstance(f.mean, CustomMean) else None
+    zb = np.empty((M, S), dtype=dt, order="F")
+    xg = _points_grad(fx0.x_kind, N, D, dt) if inputs else None  # the points go in point-major
+    xsg = _points_grad(fx.x_kind, M, D, dt) if inputs else None
+    eng.check(eng.L.agp_post_rand_grad(p.data.C.h, cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), M, C.byref(ms), C.byref(ns),
+                                       cabi.ptr(Zf), S, cabi.ptr(Ob), g.ctypes.data_as(C.POINTER(C.c_double)),
+                                       cabi.ptr(nd), cabi.ptr(md), cabi.ptr(yb), cabi.ptr(xg), cabi.ptr(nsd),
+                                       cabi.ptr(msd), cabi.ptr(zb), cabi.ptr(xsg)))
+    res = _grad_result(g, flat, k, D, f.mean, nd, md)
+    res["y"] = yb
+    res["noise_s"] = nsd.astype(np.float64) if np.ndim(fx.s2) != 0 else float(np.sum(nsd, dtype=np.float64))
+    if msd is not None:
+        res["mean_s_v"] = msd.astype(np.float64)
+    res["Z"] = zb[:, 0].copy() if ndim == 1 else zb
+    if inputs:
+        res["x"], res["xs"] = xg, xsg
+    return (out[:, 0].copy() if ndim == 1 else out), res
+
+
 def _post_call(p: PosteriorGP, pts: _Points, s2, want_var=True, want_cov=False):
     eng = engine()
     dt = p.data.C.dtype

@@ -640,6 +640,87 @@ void forward_subst_multi(agp_ctx* ctx, const T* L, int64_t lda, const T* Dinv, i
   }
 }
 
+// B <- L^-T B: forward_subst_multi's mirror, from the last block to the first.  Block k: B_k = Dinv_k' B_k (Dinv's blocks
+// are zero above their diagonal, so the full-block product is the triangular one), then B[above] -= L[block, above]' B_k,
+// both on the tile GEMM with the L operand read k-major.  The two-level schedule keeps the forward path's outer blocks
+// of 512 rows, visited last to first: the 128-steps stay inside the outer block, and everything above it receives one
+// rank-512 update on the int8-sliced kernel, with the L panel (the block's rows, the columns above) sliced k-major.  The
+// ragged outer block (n_pad not a multiple of 512, here the first one visited) updates the rows above on the tile GEMM.
+template <typename T>
+bool backward_subst_multi_tc(agp_ctx* ctx, const T* L, int64_t lda, const T* Dinv, int64_t n_pad, T* B, int64_t ldb,
+                             int64_t ncols) {
+  cudaStream_t s = ctx->stream;
+  constexpr int GW = 4;
+  const int64_t W = (int64_t)GW * TILE;
+  const int nblk = (int)(n_pad / TILE);
+  constexpr int is_f32 = std::is_same<T, double>::value ? 0 : 1;
+  const int64_t a_rows = round_up(n_pad, TILE);
+  if (!ensure_oz(ctx, a_rows + ncols, (int)W, slices_of<T>(ctx), s) || ctx->oz.bulk != 2) return false;
+  const OzakiWs& ws = ctx->oz;
+  for (int ko = (nblk - 1) / GW * GW; ko >= 0; ko -= GW) {
+    const int k_end = (ko + GW < nblk) ? ko + GW : nblk;
+    const int64_t blk0 = (int64_t)ko * TILE;
+    for (int k = k_end - 1; k >= ko; --k) {  // in-block substitution (128-steps, rows of this outer block only)
+      T* Bk = B + (int64_t)k * TILE;
+      GemmArgs a{};
+      a.A = Dinv + (int64_t)k * TILE * TILE; a.lda = TILE; a.a_kmajor = 1;
+      a.B = Bk; a.ldb = ldb; a.b_kmajor = 1;
+      a.C = Bk; a.ldc = ldb; a.M = TILE; a.N = ncols; a.K = TILE;
+      launch_gemm<T>(a, s);
+      const int64_t rows_in = (int64_t)k * TILE - blk0;
+      if (rows_in <= 0) continue;
+      GemmArgs u{};
+      u.A = L + (int64_t)k * TILE + blk0 * lda; u.lda = lda; u.a_kmajor = 1;
+      u.B = Bk; u.ldb = ldb; u.b_kmajor = 1;
+      u.C = B + blk0; u.ldc = ldb; u.M = rows_in; u.N = ncols; u.K = TILE; u.alpha_neg = 1; u.beta_one = 1;
+      launch_gemm<T>(u, s);
+    }
+    const int64_t rows_above = blk0, Kw = (int64_t)k_end * TILE - blk0;
+    if (rows_above <= 0) continue;
+    if (Kw != W) {  // ragged outer block: finish on the tile GEMM
+      GemmArgs u{};
+      u.A = L + blk0; u.lda = lda; u.a_kmajor = 1;
+      u.B = B + blk0; u.ldb = ldb; u.b_kmajor = 1;
+      u.C = B; u.ldc = ldb; u.M = rows_above; u.N = ncols; u.K = Kw; u.alpha_neg = 1; u.beta_one = 1;
+      launch_gemm<T>(u, s);
+      continue;
+    }
+    ozaki_prepare_ex(ws, L + blk0, is_f32, 1, lda, rows_above, 0, s);
+    ozaki_prepare_ex(ws, B + blk0, is_f32, 1, ldb, ncols, a_rows, s);
+    if (ozaki_update_ex(ws, B, is_f32, ldb, rows_above, ncols, 1, -1.0, 0, 0, a_rows, 0, s) != 0) return false;
+  }
+  return true;
+}
+
+// B <- L^-T B for a n_pad x ncols block of right-hand sides (ncols multiple of 4), in place; the tensor-core schedule
+// under forward_subst_multi's rule
+template <typename T>
+void backward_subst_multi(agp_ctx* ctx, const T* L, int64_t lda, const T* Dinv, int64_t n_pad, T* B, int64_t ldb,
+                          int64_t ncols) {
+  cudaStream_t s = ctx->stream;
+  const int nblk = (int)(n_pad / TILE);
+  static const int64_t tc_min_cols = env_int64("AGP_SOLVE_TC_MIN_COLS", 512);
+  if (resolve_tensor_mode<T>(ctx, n_pad >= 2048 ? (int64_t)1 << 20 : 0) == 1 && n_pad >= 2048 && ncols % TILE == 0 &&
+      ncols >= tc_min_cols) {
+    if (backward_subst_multi_tc<T>(ctx, L, lda, Dinv, n_pad, B, ldb, ncols)) return;
+  }
+  for (int k = nblk - 1; k >= 0; --k) {
+    T* Bk = B + (int64_t)k * TILE;
+    GemmArgs a{};
+    a.A = Dinv + (int64_t)k * TILE * TILE; a.lda = TILE; a.a_kmajor = 1;
+    a.B = Bk; a.ldb = ldb; a.b_kmajor = 1;
+    a.C = Bk; a.ldc = ldb; a.M = TILE; a.N = ncols; a.K = TILE;
+    launch_gemm<T>(a, s);
+    const int64_t rows_above = (int64_t)k * TILE;
+    if (rows_above <= 0) continue;
+    GemmArgs u{};
+    u.A = L + (int64_t)k * TILE; u.lda = lda; u.a_kmajor = 1;
+    u.B = Bk; u.ldb = ldb; u.b_kmajor = 1;
+    u.C = B; u.ldc = ldb; u.M = rows_above; u.N = ncols; u.K = TILE; u.alpha_neg = 1; u.beta_one = 1;
+    launch_gemm<T>(u, s);
+  }
+}
+
 template <typename T>
 void fill_gram_params(GramParams& gp, const agp_kernel* k, int symmetric, int lower_only, int64_t va, int64_t vb,
                       const agp_noise* noise, const T* noise_v_dev, const CompState* comp = nullptr) {
@@ -1531,6 +1612,112 @@ int post_logpdf_grad_cols_impl(agp_post* p, const agp_mean* mean, const void* Y,
   return AGP_OK;
 }
 
+// extra product columns of the posterior gradients' blocks: [.. alpha], [.. mubar], the -beta' row (one used, 16 keeps
+// alignment)
+constexpr int64_t POST_XK = 16;
+
+// The training side shared by agp_post_pred_logpdf_grad and agp_post_rand_grad, from the test side's cotangents.  On
+// entry: Ws (m_pad x (m_pad + POST_XK)) holds -2 Sigmabar in both triangles of its first m_pad columns and mubar in
+// column m_pad, zero elsewhere; P (n_pad x (m_pad + POST_XK)) holds P = C^-1 K_xs in its first m_pad columns (padding
+// rows and columns zero).  The tail puts alpha into column m_pad of P, forms beta = P mubar (ybar = beta, mbar = -beta)
+// and, with want_red, the stacked W over [x; x*] (the comment of post_pred_logpdf_grad_impl) and its reductions, split
+// into the training and the test outputs; grad_out[3] and [4] are the training noise and the ConstMean entries.
+template <typename T>
+int post_pred_tail(agp_post* p, Scratch& sc, int layout, const T* Xst, int64_t M, const T* Ws, T* P, bool want_red,
+                   double* grad_out, void* noise_diag_out, void* mean_diag_out, void* y_bar_out, void* x_grad_out,
+                   void* noise_s_diag_out, void* xs_grad_out) {
+  agp_ctx* ctx = p->ctx;
+  cudaStream_t s = ctx->stream;
+  const int64_t N = p->n, n_pad = p->n_pad, m_pad = round_up(M, TILE);
+  const int D = p->D;
+  constexpr int64_t XK = POST_XK;
+  const T* mubar = Ws + m_pad * m_pad;
+  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  void* tmp = nullptr;
+  int rc = AGP_OK;
+  CK(cudaMemsetAsync(P + n_pad * m_pad, 0, (size_t)n_pad * XK * sizeof(T), s));
+  CK(cudaMemcpyAsync(P + n_pad * m_pad, p->alpha, (size_t)N * sizeof(T), cudaMemcpyDeviceToDevice, s));
+  CK(sc.alloc(&tmp, (size_t)n_pad * 2 * sizeof(T)));
+  T* beta = (T*)tmp;
+  T* nbeta = beta + n_pad;
+  CK(cudaMemsetAsync(beta, 0, (size_t)n_pad * 2 * sizeof(T), s));
+  launch_gemv_n_acc<T>(P, n_pad, N, M, mubar, beta, s);
+  CK(cudaMemcpyAsync(nbeta, beta, (size_t)n_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+  launch_scale<T>(nbeta, n_pad, -1.0, s);
+  rc = download<T>(ctx, y_bar_out, beta, (size_t)N, false);
+  if (rc) return rc;
+  rc = download<T>(ctx, mean_diag_out, nbeta, (size_t)N, false);
+  if (rc) return rc;
+  if (want_red) {
+    const int64_t Lst = n_pad + m_pad, ldw = Lst + XK;
+    CK(sc.alloc(&tmp, (size_t)ldw * Lst * sizeof(T)));
+    T* Wst = (T*)tmp;
+    {
+      GemmArgs g{};  // -Kbar_sx = -[Ws mubar][P alpha]' into rows n_pad.. of the first n_pad columns
+      g.A = Ws; g.lda = m_pad; g.a_kmajor = 0;
+      g.B = P; g.ldb = n_pad; g.b_kmajor = 0;
+      g.C = Wst + n_pad; g.ldc = ldw; g.M = m_pad; g.N = n_pad; g.K = m_pad + XK; g.alpha_neg = 1;
+      launch_gemm<T>(g, s);
+    }
+    CK(cudaMemset2DAsync(Wst + Lst, (size_t)ldw * sizeof(T), 0, (size_t)XK * sizeof(T), (size_t)n_pad, s));
+    CK(cudaMemcpy2DAsync(Wst + Lst, (size_t)ldw * sizeof(T), nbeta, sizeof(T), sizeof(T), (size_t)n_pad,
+                         cudaMemcpyDeviceToDevice, s));  // the -beta' row under -Kbar_sx
+    {
+      GemmArgs g{};  // -2 Cbar = -[P alpha][-Kbar_sx; -beta'], lower tiles
+      g.A = P; g.lda = n_pad; g.a_kmajor = 0;
+      g.B = Wst + n_pad; g.ldb = ldw; g.b_kmajor = 1;
+      g.C = Wst; g.ldc = ldw; g.M = n_pad; g.N = n_pad; g.K = m_pad + XK; g.alpha_neg = 1; g.lower_only = 1;
+      launch_gemm<T>(g, s);
+    }
+    launch_copy2d<T>(Ws, m_pad, Wst + n_pad + n_pad * ldw, ldw, m_pad, m_pad, s);  // -2 Sigmabar
+    CK(sc.alloc(&tmp, (size_t)Lst * (D + 1) * sizeof(T)));
+    T* Xcat = (T*)tmp;  // [x; x*] point-major, then alpha = 0
+    T* zalpha = Xcat + Lst * D;
+    CK(cudaMemcpyAsync(Xcat, p->Xt, (size_t)n_pad * D * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemcpyAsync(Xcat + n_pad * D, Xst, (size_t)m_pad * D * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    CK(cudaMemsetAsync(zalpha, 0, (size_t)Lst * sizeof(T), s));
+    const bool want_diag = grad_out || noise_diag_out || noise_s_diag_out;
+    const bool want_x = x_grad_out || xs_grad_out;
+    T *nd = nullptr, *xg = nullptr;
+    if (want_diag) { CK(sc.alloc(&tmp, (size_t)Lst * sizeof(T))); nd = (T*)tmp; }
+    if (want_x) { CK(sc.alloc(&tmp, (size_t)Lst * D * sizeof(T))); xg = (T*)tmp; }
+    const bool saved = ctx->out_dev_override;
+    ctx->out_dev_override = true;  // the stacked outputs stay on the device and are split below
+    rc = grad_reductions_on<T>(p, sc, Xcat, Lst, Lst, Wst, ldw, zalpha, grad_out, nd, layout, xg);
+    ctx->out_dev_override = saved;
+    if (rc) return rc;
+    rc = download<T>(ctx, noise_diag_out, nd, (size_t)N, false);
+    if (rc) return rc;
+    rc = download<T>(ctx, noise_s_diag_out, want_diag ? nd + n_pad : nullptr, (size_t)M, false);
+    if (rc) return rc;
+    // the stacked input gradient in `layout`: point-major rows [0, N) and [n_pad, n_pad + M); feature-major columns
+    auto split_x = [&](void* out, int64_t off, int64_t cnt) -> int {
+      if (!out) return AGP_OK;
+      if (layout == AGP_POINT_MAJOR)
+        CK(cudaMemcpyAsync(out, xg + off * D, (size_t)cnt * D * sizeof(T), kout, s));
+      else
+        CK(cudaMemcpy2DAsync(out, (size_t)cnt * sizeof(T), xg + off, (size_t)Lst * sizeof(T), (size_t)cnt * sizeof(T),
+                             (size_t)D, kout, s));
+      return AGP_OK;
+    };
+    rc = split_x(x_grad_out, 0, N);
+    if (rc) return rc;
+    rc = split_x(xs_grad_out, n_pad, M);
+    if (rc) return rc;
+    if (grad_out) {  // d/d sigma^2 = sum_i Cbar_ii and d/d ConstMean c = sum mubar - sum beta
+      double sn = 0.0, sm = 0.0, sb = 0.0;
+      rc = host_sum<T>(ctx, nd, N, &sn); if (rc) return rc;
+      rc = host_sum<T>(ctx, beta, N, &sb); if (rc) return rc;
+      rc = host_sum<T>(ctx, mubar, M, &sm); if (rc) return rc;
+      grad_out[3] = sn;
+      grad_out[4] = sm - sb;
+    }
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return AGP_OK;
+}
+
 // ---- pullback of F = sum_s w_s logpdf(posterior(fx, y)(x*, Sigma*), Y*[:, s]) on a handle from agp_fit (agp.h
 // agp_post_pred_logpdf_grad).  With C = L L', alpha = C^-1 delta, A = L^-1 K_xs, P = C^-1 K_xs = V'A (V = L^-1),
 // mu* = m* + K_sx alpha, Sigma = K_ss - A'A + Sigma* = L* L*' and E = Y* - mu* 1':
@@ -1568,12 +1755,11 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
   rc = logpdf_grad_prelude<T>(p, layout);
   if (rc) return rc;
   cudaStream_t s = ctx->stream;
-  const int64_t N = p->n, n_pad = p->n_pad, m_pad = round_up(M, TILE), ldf = m_pad + TILE;
-  const int D = p->D, nblk = (int)(m_pad / TILE);
-  constexpr int64_t XK = 16;  // extra product columns: [.. alpha], [.. mubar], the -beta' row (one used, 16 keeps alignment)
+  const int64_t n_pad = p->n_pad, m_pad = round_up(M, TILE), ldf = m_pad + TILE;
+  const int nblk = (int)(m_pad / TILE);
+  constexpr int64_t XK = POST_XK;
   const bool want_red = grad_out || noise_diag_out || x_grad_out || noise_s_diag_out || xs_grad_out;
   const bool want_beta = want_red || mean_diag_out || y_bar_out;
-  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
   Scratch sc(ctx);
   void* tmp = nullptr;
 
@@ -1642,14 +1828,13 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
   auto drop = [&](void* q) { sc.release(q); cudaFreeAsync(q, s); };
   drop(Vs); drop(Lf); drop(Dinv);
 
-  // ---- training side: P = V'A with alpha in its column m_pad, beta = P mubar
+  // ---- training side: P = V'A, then the blocks and the reductions (post_pred_tail)
   if (want_beta) {
     T *V = nullptr, *unused = nullptr;
     rc = inverse_factor<T>(p, sc, false, &V, &unused);
     if (rc) return rc;
     CK(sc.alloc(&tmp, (size_t)n_pad * (m_pad + XK) * sizeof(T)));
     T* P = (T*)tmp;
-    CK(cudaMemsetAsync(P + n_pad * m_pad, 0, (size_t)n_pad * XK * sizeof(T), s));
     {
       GemmArgs g{};
       g.A = V; g.lda = n_pad; g.a_kmajor = 1;
@@ -1658,83 +1843,9 @@ int post_pred_logpdf_grad_impl(agp_post* p, int layout, const void* Xs, int64_t 
       launch_gemm<T>(g, s);
     }
     drop(V); drop(A);
-    CK(cudaMemcpyAsync(P + n_pad * m_pad, p->alpha, (size_t)N * sizeof(T), cudaMemcpyDeviceToDevice, s));
-    CK(sc.alloc(&tmp, (size_t)n_pad * 2 * sizeof(T)));
-    T* beta = (T*)tmp;
-    T* nbeta = beta + n_pad;
-    CK(cudaMemsetAsync(beta, 0, (size_t)n_pad * 2 * sizeof(T), s));
-    launch_gemv_n_acc<T>(P, n_pad, N, M, mubar, beta, s);
-    CK(cudaMemcpyAsync(nbeta, beta, (size_t)n_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
-    launch_scale<T>(nbeta, n_pad, -1.0, s);
-    rc = download<T>(ctx, y_bar_out, beta, (size_t)N, false);
+    rc = post_pred_tail<T>(p, sc, layout, Xst, M, Ws, P, want_red, grad_out, noise_diag_out, mean_diag_out, y_bar_out,
+                           x_grad_out, noise_s_diag_out, xs_grad_out);
     if (rc) return rc;
-    rc = download<T>(ctx, mean_diag_out, nbeta, (size_t)N, false);
-    if (rc) return rc;
-    if (want_red) {
-      const int64_t Lst = n_pad + m_pad, ldw = Lst + XK;
-      CK(sc.alloc(&tmp, (size_t)ldw * Lst * sizeof(T)));
-      T* Wst = (T*)tmp;
-      {
-        GemmArgs g{};  // -Kbar_sx = -[Ws mubar][P alpha]' into rows n_pad.. of the first n_pad columns
-        g.A = Ws; g.lda = m_pad; g.a_kmajor = 0;
-        g.B = P; g.ldb = n_pad; g.b_kmajor = 0;
-        g.C = Wst + n_pad; g.ldc = ldw; g.M = m_pad; g.N = n_pad; g.K = m_pad + XK; g.alpha_neg = 1;
-        launch_gemm<T>(g, s);
-      }
-      CK(cudaMemset2DAsync(Wst + Lst, (size_t)ldw * sizeof(T), 0, (size_t)XK * sizeof(T), (size_t)n_pad, s));
-      CK(cudaMemcpy2DAsync(Wst + Lst, (size_t)ldw * sizeof(T), nbeta, sizeof(T), sizeof(T), (size_t)n_pad,
-                           cudaMemcpyDeviceToDevice, s));  // the -beta' row under -Kbar_sx
-      {
-        GemmArgs g{};  // -2 Cbar = -[P alpha][-Kbar_sx; -beta'], lower tiles
-        g.A = P; g.lda = n_pad; g.a_kmajor = 0;
-        g.B = Wst + n_pad; g.ldb = ldw; g.b_kmajor = 1;
-        g.C = Wst; g.ldc = ldw; g.M = n_pad; g.N = n_pad; g.K = m_pad + XK; g.alpha_neg = 1; g.lower_only = 1;
-        launch_gemm<T>(g, s);
-      }
-      launch_copy2d<T>(Ws, m_pad, Wst + n_pad + n_pad * ldw, ldw, m_pad, m_pad, s);  // -2 Sigmabar
-      CK(sc.alloc(&tmp, (size_t)Lst * (D + 1) * sizeof(T)));
-      T* Xcat = (T*)tmp;  // [x; x*] point-major, then alpha = 0
-      T* zalpha = Xcat + Lst * D;
-      CK(cudaMemcpyAsync(Xcat, p->Xt, (size_t)n_pad * D * sizeof(T), cudaMemcpyDeviceToDevice, s));
-      CK(cudaMemcpyAsync(Xcat + n_pad * D, Xst, (size_t)m_pad * D * sizeof(T), cudaMemcpyDeviceToDevice, s));
-      CK(cudaMemsetAsync(zalpha, 0, (size_t)Lst * sizeof(T), s));
-      const bool want_diag = grad_out || noise_diag_out || noise_s_diag_out;
-      const bool want_x = x_grad_out || xs_grad_out;
-      T *nd = nullptr, *xg = nullptr;
-      if (want_diag) { CK(sc.alloc(&tmp, (size_t)Lst * sizeof(T))); nd = (T*)tmp; }
-      if (want_x) { CK(sc.alloc(&tmp, (size_t)Lst * D * sizeof(T))); xg = (T*)tmp; }
-      const bool saved = ctx->out_dev_override;
-      ctx->out_dev_override = true;  // the stacked outputs stay on the device and are split below
-      rc = grad_reductions_on<T>(p, sc, Xcat, Lst, Lst, Wst, ldw, zalpha, grad_out, nd, layout, xg);
-      ctx->out_dev_override = saved;
-      if (rc) return rc;
-      rc = download<T>(ctx, noise_diag_out, nd, (size_t)N, false);
-      if (rc) return rc;
-      rc = download<T>(ctx, noise_s_diag_out, want_diag ? nd + n_pad : nullptr, (size_t)M, false);
-      if (rc) return rc;
-      // the stacked input gradient in `layout`: point-major rows [0, N) and [n_pad, n_pad + M); feature-major columns
-      auto split_x = [&](void* out, int64_t off, int64_t cnt) -> int {
-        if (!out) return AGP_OK;
-        if (layout == AGP_POINT_MAJOR)
-          CK(cudaMemcpyAsync(out, xg + off * D, (size_t)cnt * D * sizeof(T), kout, s));
-        else
-          CK(cudaMemcpy2DAsync(out, (size_t)cnt * sizeof(T), xg + off, (size_t)Lst * sizeof(T), (size_t)cnt * sizeof(T),
-                               (size_t)D, kout, s));
-        return AGP_OK;
-      };
-      rc = split_x(x_grad_out, 0, N);
-      if (rc) return rc;
-      rc = split_x(xs_grad_out, n_pad, M);
-      if (rc) return rc;
-      if (grad_out) {  // d/d sigma^2 = sum_i Cbar_ii and d/d ConstMean c = sum mubar - sum beta
-        double sn = 0.0, sm = 0.0, sb = 0.0;
-        rc = host_sum<T>(ctx, nd, N, &sn); if (rc) return rc;
-        rc = host_sum<T>(ctx, beta, N, &sb); if (rc) return rc;
-        rc = host_sum<T>(ctx, mubar, M, &sm); if (rc) return rc;
-        grad_out[3] = sn;
-        grad_out[4] = sm - sb;
-      }
-    }
   }
   CK(cudaStreamSynchronize(s));
   CK(cudaGetLastError());
@@ -1989,10 +2100,55 @@ int rand_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp
   return AGP_OK;
 }
 
+// The pullback of a Cholesky sample out = L Z (C = L L', n rows, n_pad padded, L of leading dimension lda) at its
+// cotangent Obar, shared by agp_rand_grad and agp_post_rand_grad.  Od and Zd hold Obar and Z (n_pad x s_pad, padding
+// zeroed).  Into the caller's buffers:
+//   Zb = L' Obar;  rowsum_i = sum_s Obar_is (fp64, in order);
+//   and, when V = L^-1 (leading dimension n_pad) is given: Q = the lower triangle of Zb Z' mirrored, into Wout;
+//   W1 = Q V, into Lt;  -V' W1 = -V'QV into Wout (its lower tiles only with lower_only, else both triangles).
+// Lt (L', then W1) and Wout are n_pad x n_pad.  L' is taken whole from the factor (its storage above the diagonal blocks
+// is not zeroed).
+template <typename T>
+void sample_pullback(agp_ctx* ctx, const T* L, int64_t lda, const T* V, int64_t n, int64_t n_pad, int S, int64_t s_pad,
+                     const T* Od, const T* Zd, T* Zb, double* rowsum, T* Lt, T* Wout, bool lower_only) {
+  cudaStream_t s = ctx->stream;
+  launch_rowsum<T>(Od, n_pad, n, S, rowsum, s);
+  launch_export_upper<T>(L, lda, n_pad, Lt, n_pad, s);
+  {
+    GemmArgs g{};
+    g.A = Lt; g.lda = n_pad; g.a_kmajor = 0;
+    g.B = Od; g.ldb = n_pad; g.b_kmajor = 1;
+    g.C = Zb; g.ldc = n_pad; g.M = n_pad; g.N = s_pad; g.K = n_pad;
+    launch_gemm<T>(g, s);
+  }
+  if (!V) return;
+  {
+    GemmArgs g{};  // Q = Zbar Z', lower tiles (K = S), then mirrored
+    g.A = Zb; g.lda = n_pad; g.a_kmajor = 0;
+    g.B = Zd; g.ldb = n_pad; g.b_kmajor = 0;
+    g.C = Wout; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = s_pad; g.lower_only = 1;
+    launch_gemm<T>(g, s);
+    launch_symmetrize_lower<T>(Wout, n_pad, n_pad, s);
+  }
+  {
+    GemmArgs g{};  // W1 = Q V
+    g.A = Wout; g.lda = n_pad; g.a_kmajor = 0;
+    g.B = V; g.ldb = n_pad; g.b_kmajor = 1;
+    g.C = Lt; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad;
+    launch_gemm<T>(g, s);
+  }
+  {
+    GemmArgs g{};  // -V' W1
+    g.A = V; g.lda = n_pad; g.a_kmajor = 1;
+    g.B = Lt; g.ldb = n_pad; g.b_kmajor = 1;
+    g.C = Wout; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = lower_only ? 1 : 0; g.alpha_neg = 1;
+    launch_gemm<T>(g, s);
+  }
+}
+
 // ---- pullback of rand: out = m + L Z, C = K + Sigma_y = L L' (agp.h agp_rand_grad).  In fp64 whatever the caller's dtype
 // (rand_grad_f32).  The factor comes from the factor-only fit as an agp_post, so the reductions of the logpdf gradient
-// (grad_reductions) run on it with alpha = 0 and Cinv = -V'QV:
-//   Zbar = L' Obar;  Q = the lower triangle of Zbar Z' mirrored;  V = L^-1;  W1 = Q V;  -V' W1 into lower tiles.
+// (grad_reductions) run on it with alpha = 0 and Cinv = -V'QV from sample_pullback (-2 Cbar, lower tiles).
 // Three n_pad x n_pad buffers besides the factor; ~4 N^3 flop (the substitution N^3, Q V 2 N^3, the lower half of V'W1 N^3).
 int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_noise* noise, int layout, const void* X,
                   int64_t N, int D, const void* Z, int S, const void* out_bar, double* grad_out, void* noise_diag_out,
@@ -2028,42 +2184,11 @@ int rand_grad_f64(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
     CK(cudaMemcpy2DAsync(Od, (size_t)n_pad * sizeof(T), out_bar, (size_t)N * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kin, s));
     CK(cudaMemcpy2DAsync(Zd, (size_t)n_pad * sizeof(T), Z, (size_t)N * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kin, s));
   }
-  // mbar_i = sum_s Obar_is
-  launch_rowsum<T>(Od, n_pad, N, S, mbar, s);
-  // Zbar = L' Obar: L' taken whole from the factor (its storage above the diagonal blocks is not zeroed)
-  launch_export_upper<T>((const T*)p->L, p->lda, n_pad, B1, n_pad, s);
-  {
-    GemmArgs g{};
-    g.A = B1; g.lda = n_pad; g.a_kmajor = 0;
-    g.B = Od; g.ldb = n_pad; g.b_kmajor = 1;
-    g.C = Zb; g.ldc = n_pad; g.M = n_pad; g.N = s_pad; g.K = n_pad;
-    launch_gemm<T>(g, s);
-  }
+  // mbar_i = sum_s Obar_is, Zbar = L' Obar and, for the reductions, -V'QV = -2 Cbar (lower tiles) into B2
+  sample_pullback<T>(ctx, (const T*)p->L, p->lda, V, N, n_pad, S, s_pad, Od, Zd, Zb, mbar, B1, B2, true);
   if (z_bar_out && S > 0)
     CK(cudaMemcpy2DAsync(z_bar_out, (size_t)N * sizeof(T), Zb, (size_t)n_pad * sizeof(T), (size_t)N * sizeof(T), (size_t)S, kout, s));
   if (want_c) {
-    {
-      GemmArgs g{};  // Q = Zbar Z', lower tiles (K = S), then mirrored
-      g.A = Zb; g.lda = n_pad; g.a_kmajor = 0;
-      g.B = Zd; g.ldb = n_pad; g.b_kmajor = 0;
-      g.C = B2; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = s_pad; g.lower_only = 1;
-      launch_gemm<T>(g, s);
-      launch_symmetrize_lower<T>(B2, n_pad, n_pad, s);
-    }
-    {
-      GemmArgs g{};  // W1 = Q V
-      g.A = B2; g.lda = n_pad; g.a_kmajor = 0;
-      g.B = V; g.ldb = n_pad; g.b_kmajor = 1;
-      g.C = B1; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad;
-      launch_gemm<T>(g, s);
-    }
-    {
-      GemmArgs g{};  // -V' W1 = -2 Cbar, lower tiles
-      g.A = V; g.lda = n_pad; g.a_kmajor = 1;
-      g.B = B1; g.ldb = n_pad; g.b_kmajor = 1;
-      g.C = B2; g.ldc = n_pad; g.M = n_pad; g.N = n_pad; g.K = n_pad; g.lower_only = 1; g.alpha_neg = 1;
-      launch_gemm<T>(g, s);
-    }
     rc = grad_reductions<T>(p, sc, B2, zero_alpha, grad_out, noise_diag_out, layout, x_grad_out);
     if (rc) return rc;
   }
@@ -2213,6 +2338,108 @@ int rand_grad_f32(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
                      out[2], out[3]);
   if (rc) return rc;
   return p.narrow();
+}
+
+// ---- pullback of rand(posterior(fx, y)(x*, Sigma*), S) on a handle from agp_fit (agp.h agp_post_rand_grad).  The forward
+// is agp_post_rand's: mu* = m* + K_sx alpha, A = L^-1 K_xs, Sigma = K_ss + Sigma* - A'A = L* L*', out = mu* 1' + L* Z.
+// The head is sample_pullback on L*: Zbar = L*' Obar, mubar = Obar 1 and -V*'QV* = -2 Sigmabar in both triangles
+// (V* = L*^-1 with its identity padding zeroed, as in the held-out gradient).  From there the training side is the
+// held-out gradient's (post_pred_tail), except that P = C^-1 K_xs = L^-T A comes from backward_subst_multi (N^2 M flop)
+// instead of V = L^-1 (N^3) and V'A: no N x N buffer is allocated besides the stacked W, and the call has no N^3 term.
+template <typename T>
+int post_rand_grad_impl(agp_post* p, int layout, const void* Xs, int64_t M, const agp_mean* mean_s,
+                        const agp_noise* noise_s, const void* Z, int S, const void* out_bar, double* grad_out,
+                        void* noise_diag_out, void* mean_diag_out, void* y_bar_out, void* x_grad_out, void* noise_s_diag_out,
+                        void* mean_s_diag_out, void* z_bar_out, void* xs_grad_out) {
+  agp_ctx* ctx = p->ctx;
+  if (S < 1) { ctx->err = "S must be >= 1"; return AGP_ERR_INVALID; }
+  if (!Z || !out_bar) { ctx->err = "Z/out_bar is NULL"; return AGP_ERR_INVALID; }
+  if (!Xs) { ctx->err = "Xs is NULL"; return AGP_ERR_INVALID; }
+  if (M <= 0) { ctx->err = "M must be positive"; return AGP_ERR_DIM_MISMATCH; }
+  agp_mean mz;
+  int rc = post_side_defaults(p, &mean_s, &noise_s, &mz);
+  if (rc) return rc;
+  rc = logpdf_grad_prelude<T>(p, layout);
+  if (rc) return rc;
+  cudaStream_t s = ctx->stream;
+  const int64_t n_pad = p->n_pad, m_pad = round_up(M, TILE), ldf = m_pad + TILE, s_pad = round_up(S, 4);
+  constexpr int64_t XK = POST_XK;
+  const bool want_red = grad_out || noise_diag_out || x_grad_out || noise_s_diag_out || xs_grad_out;
+  const bool want_beta = want_red || mean_diag_out || y_bar_out;
+  const cudaMemcpyKind kin = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  const cudaMemcpyKind kout = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost;
+  Scratch sc(ctx);
+  void* tmp = nullptr;
+  auto drop = [&](void* q) { sc.release(q); cudaFreeAsync(q, s); };
+
+  // ---- forward: mu*, A = L^-1 K_xs, Sigma = K_ss + Sigma* - A'A and its factor (agp_post_rand's)
+  T *Xst = nullptr, *A = nullptr;
+  rc = post_cross<T>(p, sc, layout, Xs, M, m_pad, &Xst, &A);
+  if (rc) return rc;
+  T *mean_d = nullptr, *noise_d = nullptr;
+  if (mean_s->kind == 2) { rc = upload<T>(ctx, sc, mean_s->v, M, true, &mean_d); if (rc) return rc; }
+  if (noise_s->kind == 1) { rc = upload<T>(ctx, sc, noise_s->v, M, true, &noise_d); if (rc) return rc; }
+  CK(sc.alloc(&tmp, (size_t)m_pad * sizeof(T)));
+  T* mu = (T*)tmp;
+  CK(cudaMemsetAsync(mu, 0, (size_t)m_pad * sizeof(T), s));
+  launch_gemv_t<T>(A, n_pad, n_pad, M, (const T*)p->alpha, mean_s->kind, mean_s->c, mean_d, mu, s);
+  forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, A, n_pad, m_pad);
+  T *Lf = nullptr, *Dinv = nullptr;
+  double* dscal = nullptr;
+  int* dinfo = nullptr;
+  rc = post_cov_factor<T>(p, sc, Xst, A, M, noise_s, noise_d, (const T*)nullptr, 0, mu, &Lf, &Dinv, &dscal, &dinfo);
+  if (rc) return rc;
+  rc = post_cov_status(ctx, dinfo);
+  if (rc) return rc;
+
+  // ---- head: Zbar, mubar (column m_pad of Ws) and, for the reductions, Ws = -2 Sigmabar
+  CK(sc.alloc(&tmp, (size_t)m_pad * m_pad * sizeof(T)));
+  T* Lt = (T*)tmp;
+  CK(sc.alloc(&tmp, (size_t)m_pad * (m_pad + XK) * sizeof(T)));
+  T* Ws = (T*)tmp;
+  T* mubar = Ws + m_pad * m_pad;
+  CK(cudaMemsetAsync(Ws, 0, (size_t)m_pad * (m_pad + XK) * sizeof(T), s));
+  T* Vs = nullptr;
+  if (want_red) {
+    CK(sc.alloc(&tmp, (size_t)m_pad * m_pad * sizeof(T)));
+    Vs = (T*)tmp;
+    CK(cudaMemsetAsync(Vs, 0, (size_t)m_pad * m_pad * sizeof(T), s));
+    launch_add_diag<T>(Vs, m_pad, M, 1.0, s);
+    forward_subst_multi<T>(ctx, (const T*)Lf, ldf, (const T*)Dinv, m_pad, Vs, m_pad, m_pad);
+  }
+  CK(sc.alloc(&tmp, (size_t)m_pad * s_pad * sizeof(T) * 3));
+  T* Od = (T*)tmp; T* Zd = Od + m_pad * s_pad; T* Zb = Zd + m_pad * s_pad;
+  CK(sc.alloc(&tmp, (size_t)m_pad * sizeof(double)));
+  double* rs = (double*)tmp;
+  CK(cudaMemsetAsync(Od, 0, (size_t)m_pad * s_pad * sizeof(T) * 2, s));  // zero padding rows / columns of Obar and Z
+  CK(cudaMemcpy2DAsync(Od, (size_t)m_pad * sizeof(T), out_bar, (size_t)M * sizeof(T), (size_t)M * sizeof(T), (size_t)S, kin, s));
+  CK(cudaMemcpy2DAsync(Zd, (size_t)m_pad * sizeof(T), Z, (size_t)M * sizeof(T), (size_t)M * sizeof(T), (size_t)S, kin, s));
+  sample_pullback<T>(ctx, (const T*)Lf, ldf, Vs, M, m_pad, S, s_pad, Od, Zd, Zb, rs, Lt, Ws, false);
+  if (std::is_same<T, double>::value)
+    CK(cudaMemcpyAsync(mubar, rs, (size_t)M * sizeof(double), cudaMemcpyDeviceToDevice, s));
+  else
+    launch_cast<double, float>(rs, (float*)mubar, M, s);
+  if (z_bar_out)
+    CK(cudaMemcpy2DAsync(z_bar_out, (size_t)M * sizeof(T), Zb, (size_t)m_pad * sizeof(T), (size_t)M * sizeof(T), (size_t)S, kout, s));
+  rc = download<T>(ctx, mean_s_diag_out, mubar, (size_t)M, false);
+  if (rc) return rc;
+  drop(Od); drop(Lt); drop(Lf); drop(Dinv);
+  if (Vs) drop(Vs);
+
+  // ---- training side: P = L^-T A with room for alpha (post_pred_tail), then the blocks and the reductions
+  if (want_beta) {
+    CK(sc.alloc(&tmp, (size_t)n_pad * (m_pad + XK) * sizeof(T)));
+    T* P = (T*)tmp;
+    CK(cudaMemcpyAsync(P, A, (size_t)n_pad * m_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    drop(A);
+    backward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, P, n_pad, m_pad);
+    rc = post_pred_tail<T>(p, sc, layout, Xst, M, Ws, P, want_red, grad_out, noise_diag_out, mean_diag_out, y_bar_out,
+                           x_grad_out, noise_s_diag_out, xs_grad_out);
+    if (rc) return rc;
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return AGP_OK;
 }
 
 template <typename T>
@@ -3429,6 +3656,20 @@ int32_t agp_post_pred_logpdf_grad(agp_post* p, int32_t layout, const void* Xs, i
                   post_pred_logpdf_grad_impl<double>(p, layout, Xs, M, mean_s, noise_s, Ys, S, lp_bar, lp_out, grad_out,
                                                      noise_diag_out, mean_diag_out, y_bar_out, x_grad_out, noise_s_diag_out,
                                                      mean_s_diag_out, ys_bar_out, xs_grad_out));
+}
+
+int32_t agp_post_rand_grad(agp_post* p, int32_t layout, const void* Xs, int64_t M, const agp_mean* mean_s,
+                           const agp_noise* noise_s, const void* Z, int32_t S, const void* out_bar, double* grad_out,
+                           void* noise_diag_out, void* mean_diag_out, void* y_bar_out, void* x_grad_out,
+                           void* noise_s_diag_out, void* mean_s_diag_out, void* z_bar_out, void* xs_grad_out) {
+  if (!p) return AGP_ERR_INVALID;
+  return DISPATCH(p->dtype,
+                  post_rand_grad_impl<float>(p, layout, Xs, M, mean_s, noise_s, Z, S, out_bar, grad_out, noise_diag_out,
+                                             mean_diag_out, y_bar_out, x_grad_out, noise_s_diag_out, mean_s_diag_out,
+                                             z_bar_out, xs_grad_out),
+                  post_rand_grad_impl<double>(p, layout, Xs, M, mean_s, noise_s, Z, S, out_bar, grad_out, noise_diag_out,
+                                              mean_diag_out, y_bar_out, x_grad_out, noise_s_diag_out, mean_s_diag_out,
+                                              z_bar_out, xs_grad_out));
 }
 
 int32_t agp_post_solve_lower(agp_post* p, const void* B, int64_t nrhs, void* V_out) {

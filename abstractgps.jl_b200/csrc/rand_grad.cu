@@ -1,4 +1,4 @@
-// rand_grad.cu -- the two small kernels of the pullback of rand(fx, S) (agp_rand_grad, agp.h).  The N^3 work of that
+// rand_grad.cu -- the two small kernels of the pullback of rand(fx, S) (agp_rand_grad and agp_post_rand_grad, agp.h).  The N^3 work of that
 // pullback runs on the tile GEMM and the forward substitution; what is left is
 //   - Q: the symmetric matrix whose lower triangle (diagonal included) is that of Zbar Z'.  The lower-only GEMM writes
 //     the lower tiles; symmetrize_lower copies the strict lower triangle onto the upper one.
@@ -59,3 +59,6 @@ void launch_rowsum(const T* A, int64_t lda, int64_t n, int S, double* out, cudaS
 
 template void launch_symmetrize_lower<double>(double*, int64_t, int64_t, cudaStream_t);
 template void launch_rowsum<double>(const double*, int64_t, int64_t, int, double*, cudaStream_t);
+// agp_post_rand_grad runs fp32 handles in fp32
+template void launch_symmetrize_lower<float>(float*, int64_t, int64_t, cudaStream_t);
+template void launch_rowsum<float>(const float*, int64_t, int64_t, int, double*, cudaStream_t);

@@ -288,6 +288,47 @@ int32_t agp_post_pred_logpdf_grad(agp_post* p, int32_t layout, const void* Xs, i
                                   double* grad_out, void* noise_diag_out, void* mean_diag_out, void* y_bar_out,
                                   void* x_grad_out, void* noise_s_diag_out, void* mean_s_diag_out, void* ys_bar_out,
                                   void* xs_grad_out);
+/* Pullback of agp_post_rand at the same arguments: what reverse-mode AD returns through the reference's
+ * rand(rng, posterior(fx, y)(x*, Sigma*), S) (test/finite_gp_projection.jl:105-127 over a posterior), for Monte Carlo
+ * acquisition functions (q-EI, q-NEI, q-KG) and losses built on reparameterised posterior samples.  p must come straight
+ * from agp_fit.  With C = K_xx + Sigma_y = L L', alpha = C^-1 (y - m), A = L^-1 K_xs, P = C^-1 K_xs = L^-T A,
+ * mu* = m* + K_sx alpha, Sigma = K_ss + Sigma* - A'A = L* L*', out = mu* 1' + L* Z, Obar the cotangent of out (M x S
+ * column-major, like Z) and V* = L*^-1:
+ *   z_bar = L*' Obar,  mubar = Obar 1,  Sigmabar = 1/2 V*' Q V*,  Q symmetric with the lower triangle (diagonal included)
+ *           of z_bar Z'   (agp_rand_grad's Cholesky pullback, applied to L*)
+ * and from Sigmabar and mubar the formulas of agp_post_pred_logpdf_grad, unchanged:
+ *   Kbar_sx = mubar alpha' - 2 Sigmabar P',  Cbar = P Sigmabar P' - 1/2 (beta alpha' + alpha beta'),  beta = P mubar,
+ *   ybar = beta,  mbar = -beta at x,  mbar* = mubar,  d/d sigma_i^2 = Cbar_ii,  d/d sigma*_m^2 = Sigmabar_mm,
+ *   d/d ConstMean c = sum mubar - sum beta,  both input gradients from the stacked W over [x; x*].
+ * Inputs: Xs, mean_s, noise_s as agp_post_rand's (NULL mean_s: the handle's zero or constant mean; NULL noise_s: 1e-18),
+ * Z and out_bar (M x S each, any S >= 1).
+ * Outputs, each may be NULL and its work is then skipped: grad_out (double, the layout of agp_post_logpdf_grad: 5 + D for
+ * a single kernel, agp_post_grad_len(p) for a composite; [3] d/d sigma^2 of the training scalar noise, [4] d/d ConstMean
+ * c), noise_diag_out, mean_diag_out and y_bar_out (N values each), x_grad_out (N x D in `layout`), noise_s_diag_out and
+ * mean_s_diag_out (M values each), z_bar_out (M x S) and xs_grad_out (M x D in `layout`).  Every output but grad_out has
+ * the handle's dtype; under AGP_MEM_DEVICE, Xs, Z, out_bar and those outputs are DEVICE pointers.  The gradient of a
+ * scalar test noise is the sum of noise_s_diag_out.
+ * Cost: the forward of agp_post_rand (N^2 M for A, M^3 / 3 for the factor of Sigma, M^2 S for the sample), then M^2 S for
+ * z_bar and, when a kernel, noise, x or x* output is asked for, ~5 M^3 for the head (V* M^3 / 3 .. M^3, Q V* 2 M^3,
+ * V*' (Q V*) 2 M^3); when any training-side output is asked for, N^2 M for P (a multi-column backward substitution on
+ * L, on the int8-sliced tensor cores above the forward substitution's threshold), then 2 N M^2 for Kbar_sx, N^2 M for
+ * Cbar (the lower half) and the reductions over (N + M)^2 / 2 pairs.  There is no N^3 term: V = L^-1 is never formed.
+ * Memory, besides the handle, in elements of the handle's dtype: about NM + 4 M^2 + 3 MS for the forward and the head,
+ * then NM + M^2 + (N + M)^2 for P, Sigmabar and the stacked W (which also holds the 2 NM elements of its unused upper
+ * block); no other N x N buffer is allocated.
+ * Arithmetic: the handle's dtype for the factors, V*, P and the products, fp64 for the row sums of Obar and the
+ * reductions (as agp_post_pred_logpdf_grad; an fp32 handle keeps only its transformed fp32 points, so there is no fp64
+ * refit).  The fp32 error grows with cond(C) and cond(Sigma) (DESIGN s6).
+ * Determinism: every per-point output, z_bar_out and grad_out[3], grad_out[4] are formed in a fixed order (two calls give
+ * the same bits); the other entries of grad_out leave their CTAs through fp64 atomics and agree to rounding.
+ * Errors: a bad layout, S < 1, a NULL Xs, Z or out_bar, or a vector mean / noise with a NULL v: AGP_ERR_INVALID; M < 1:
+ * AGP_ERR_DIM_MISMATCH; an extended handle: AGP_ERR_UNSUPPORTED; a Sigma that is not positive definite:
+ * AGP_ERR_NOT_POSDEF (agp_last_info gives the pivot); a failed device allocation: AGP_ERR_CUDA.  VFE posteriors are not
+ * covered. */
+int32_t agp_post_rand_grad(agp_post* p, int32_t layout, const void* Xs, int64_t M, const agp_mean* mean_s,
+                           const agp_noise* noise_s, const void* Z, int32_t S, const void* out_bar, double* grad_out,
+                           void* noise_diag_out, void* mean_diag_out, void* y_bar_out, void* x_grad_out,
+                           void* noise_s_diag_out, void* mean_s_diag_out, void* z_bar_out, void* xs_grad_out);
 /* number of doubles agp_post_logpdf_grad writes: 5 + D for a single kernel, the layout above for a composite */
 int64_t agp_post_grad_len(const agp_post* p);
 /* V = U' \ B (N x nrhs, column-major): backs Xt_invA_X / diag_Xt_invA_X / Xt_invA_Y /

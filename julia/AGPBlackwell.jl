@@ -290,17 +290,7 @@ function logpdf(fx::DevPostFiniteGP{T}, Y::AbstractVecOrMat{<:Real}) where {T}
     end
     return Y isa AbstractVector ? lp[1] : lp
 end
-function Random.rand(rng::Random.AbstractRNG, fx::DevPostFiniteGP{T}, S::Int) where {T}
-    p = fx.f; c = ctx(); Xs, layout, D = points(fx.x); M = length(fx)
-    Z = randn(rng, T, M, S); out = similar(Z)
-    ms, k2 = mean_spec(p.prior.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
-    lock(c.lock) do
-        GC.@preserve Xs k2 k3 check(c, ccall((:agp_post_rand, libagp), Int32,
-            (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Int64, Ref{AgpMean}, Ref{AgpNoise}, Ptr{Cvoid}, Int32, Ptr{Cvoid}),
-            p.data.C.h, layout, Xs, M, ms, ns, Z, S, out))
-    end
-    return out
-end
+Random.rand(rng::Random.AbstractRNG, fx::DevPostFiniteGP{T}, S::Int) where {T} = post_rand_primal(rng, fx, S, false)[1]
 function posterior(fx::DevPostFiniteGP{T}, y::AbstractVector{<:Real}) where {T}
     p = fx.f; c = ctx(); X2, layout, D = points(fx.x); N2 = length(fx); N1 = p.data.C.n
     yv = convert(Vector{T}, y); α = Vector{T}(undef, N1 + N2); post = Ref{Ptr{Cvoid}}(C_NULL)
@@ -726,6 +716,77 @@ function CRC.rrule(config::CRC.RuleConfig{>:CRC.HasReverseMode}, ::typeof(Random
     end
     return out, rand_pullback
 end
+
+# ---- reverse-mode rule for rand(rng, fx, S) over a device posterior (Monte Carlo acquisition functions: q-EI, q-NEI,
+# q-KG differentiate reparameterised samples μ* + L* Z with respect to x* and the hyper-parameters) --------------------
+# The forward pass is the primal method's (post_rand_primal: Z from the caller's rng, then agp_post_rand); the pullback
+# makes ONE agp_post_rand_grad call at the same Z.  The tangents are those of the logpdf-over-posterior rule: the kernel, data.x,
+# data.δ = ȳ and data.C in the DevPosterior's tangent (the posterior rule routes them on), the test points, noise and
+# the prior mean's test side in fx's.  A CustomMean prior goes through AD of `mean_split_post_rand`: the closure's values
+# at x* plus a device sample with a zero test mean (`zero_mean_post_rand`, whose rule is the same pullback).
+function post_rand_primal(rng, fx::DevPostFiniteGP{T}, S::Int, zero_mean::Bool) where {T}
+    p = fx.f; c = ctx(); Xs, layout, D = points(fx.x); M = length(fx)
+    Z = randn(rng, T, M, S); out = similar(Z)
+    ms, k2 = zero_mean ? mean_spec(AbstractGPs.ZeroMean(), fx.x, T) : mean_spec(p.prior.mean, fx.x, T)
+    ns, k3 = noise_spec(fx.Σy, T)
+    lock(c.lock) do
+        GC.@preserve Xs k2 k3 check(c, ccall((:agp_post_rand, libagp), Int32,
+            (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Int64, Ref{AgpMean}, Ref{AgpNoise}, Ptr{Cvoid}, Int32, Ptr{Cvoid}),
+            p.data.C.h, layout, Xs, M, ms, ns, Z, S, out))
+    end
+    return out, Z, ms, k2, ns, k3
+end
+
+zero_mean_post_rand(rng, fx::DevPostFiniteGP, S::Int) = post_rand_primal(rng, fx, S, true)[1]
+mean_split_post_rand(rng, fx::DevPostFiniteGP{T}, S::Int) where {T} =
+    T.(AbstractGPs.mean_vector(fx.f.prior.mean, fx.x)) .+ zero_mean_post_rand(rng, fx, S)
+
+function post_rand_rrule(rng, fx::DevPostFiniteGP{T}, S::Int, zero_mean::Bool) where {T}
+    p = fx.f
+    out, Z, ms, k2, ns, k3 = post_rand_primal(rng, fx, S, zero_mean)
+    c = ctx(); Xs, layout, D = points(fx.x); M = length(fx)
+    X, xlayout, _ = points(p.data.x); N = p.data.C.n
+    composite = !supported(p.prior)
+    function post_rand_pullback(Δ)
+        Δ = CRC.unthunk(Δ)
+        Δ isa CRC.AbstractZero && return CRC.NoTangent(), CRC.NoTangent(), CRC.ZeroTangent(), CRC.NoTangent()
+        Ō = convert(Matrix{T}, Δ)
+        glen = composite ? ccall((:agp_post_grad_len, libagp), Int64, (Ptr{Cvoid},), p.data.C.h) : 5 + D
+        g = Vector{Float64}(undef, glen); nd = Vector{T}(undef, N); ȳ = Vector{T}(undef, N)
+        xg = X isa AbstractVector || xlayout == layout ? similar(X, T) : similar(permutedims(X), T)
+        nsd = Vector{T}(undef, M); xsg = similar(Xs, T)
+        lock(c.lock) do
+            GC.@preserve Xs Z Ō g nd ȳ xg nsd xsg k2 k3 check(c, ccall((:agp_post_rand_grad, libagp), Int32,
+                (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Int64, Ref{AgpMean}, Ref{AgpNoise}, Ptr{Cvoid}, Int32, Ptr{Cvoid}, Ptr{Float64},
+                 Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid}),
+                p.data.C.h, layout, Xs, M, ms, ns, Z, S, Ō, g, nd, C_NULL, ȳ, xg, nsd, C_NULL, C_NULL, xsg))
+        end
+        # grad_out[5] is d/dc through both sides; the prior mean's tangent keeps the test side, data.δ carries the rest
+        gs = (variance=g[1], scale=g[2], linear_c=g[3], noise=g[4], mean_c=g[5] + sum(ȳ), ard=g[6:end], noise_diag=nd)
+        if composite
+            kt = ctangent(p.prior.kernel, Int[], composite_grads(p.prior.kernel, D, g), 1.0)
+        else
+            _, var, _, wt = flat(p.prior.kernel)
+            kt = kernel_tangent(p.prior.kernel, gs, var, wt === nothing ? 1.0 : wt)
+        end
+        m̄ = zero_mean ? CRC.NoTangent() : mean_tangent(p.prior.mean, gs)
+        p̄rior = CRC.Tangent{typeof(p.prior)}(; mean=m̄, kernel=kt)
+        d̄ata = CRC.Tangent{typeof(p.data)}(; C=(noise=g[4], noise_diag=nd),
+                                            x=x_tangent(p.data.x, as_storage(xg, X, layout, xlayout)), δ=ȳ)
+        f̄ = CRC.Tangent{typeof(p)}(; prior=p̄rior, data=d̄ata)
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, xsg), Σy=noise_tangent(fx.Σy, (noise=sum(nsd), noise_diag=nsd)))
+        return CRC.NoTangent(), CRC.NoTangent(), f̄x, CRC.NoTangent()
+    end
+    return out, post_rand_pullback
+end
+
+function CRC.rrule(config::CRC.RuleConfig{>:CRC.HasReverseMode}, ::typeof(Random.rand), rng::Random.AbstractRNG,
+                   fx::DevPostFiniteGP{T}, S::Int) where {T}
+    fx.f.prior.mean isa AbstractGPs.CustomMean && return CRC.rrule_via_ad(config, mean_split_post_rand, rng, fx, S)
+    return post_rand_rrule(rng, fx, S, false)
+end
+CRC.rrule(::typeof(zero_mean_post_rand), rng::Random.AbstractRNG, fx::DevPostFiniteGP, S::Int) =
+    post_rand_rrule(rng, fx, S, true)
 
 # ---- reverse-mode rules for the VFE objectives: elbo(VFE(fz), fx, y) and approx_log_evidence(VFE | DTC, fx, y) ---------
 # (src/sparse_approximations.jl:248-254, :282-286).  One agp_vfe_elbo_grad_x call returns the value, the kernel / noise /
