@@ -113,6 +113,8 @@ SIGNATURES = {
                                          C.c_int32, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_double]),
     "agp_debug_ozaki_syrk_map": (C.c_int32, [_P, _P, C.c_int64, _P, C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int32,
                                              C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64]),
+    "agp_debug_ozaki8": (C.c_int32, [_P, _P, C.c_int64, _P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64,
+                                     C.c_int64, C.c_int64, C.c_int32, C.c_double, C.c_int64, C.c_int64, C.c_int64, C.c_int64]),
     "agp_bc_owner": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "agp_bc_local_tiles": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
 }

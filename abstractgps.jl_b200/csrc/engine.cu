@@ -50,7 +50,7 @@ struct agp_ctx {
   OzakiWs oz2{};           // second slice buffer of the pipelined distributed schedule (panel k+1 is sliced while rest(k) runs)
   int64_t oz_rows = 0, oz2_rows = 0;
   cudaStream_t stream_comm = nullptr;  // panel broadcasts of the pipelined distributed schedule
-  int oz_S = 7;
+  int oz_S = 6;             // ozaki_slices: 6 = six 8-bit digits in the factorisation (slice_format), 5, 7, 8 = 7-bit slices
   int oz_chunk = 16;        // bounded-CTA size (tiles) of the rest updates that run beside a higher-priority stream; 0 = persistent
   int oz_S32 = 4;          // slices of the fp32 operands (4 x 7 bits >= the 24-bit significand)
 };
@@ -391,23 +391,34 @@ static int resolve_fp32_mode(const agp_ctx* ctx, int64_t n_pad) {
 template <typename T> static int resolve_tensor_mode(const agp_ctx* ctx, int64_t n_pad) {
   return std::is_same<T, double>::value ? resolve_fp64_mode(ctx, n_pad) : resolve_fp32_mode(ctx, n_pad);
 }
-template <typename T> static int slices_of(const agp_ctx* ctx) { return std::is_same<T, double>::value ? ctx->oz_S : ctx->oz_S32; }
-// (re)size the cached slice workspace: rows x K bytes per slice, S slices
-static bool ensure_oz2(agp_ctx* ctx, int64_t rows, int K, int S, cudaStream_t s) {  // second cached workspace (long-K products)
-  if (!ctx->oz2.SL || ctx->oz2.K != K || ctx->oz2_rows < rows || ctx->oz2.S != S) {
-    if (ctx->oz2.SL) ozaki_ws_destroy(&ctx->oz2, s);
-    if (ozaki_ws_create(&ctx->oz2, rows, K, S, s) == 0) ctx->oz2_rows = rows;
-    else { memset(&ctx->oz2, 0, sizeof(ctx->oz2)); ctx->oz2_rows = 0; }
-  }
-  return ctx->oz2.SL != nullptr;
+// slice format of a product with K-byte slice rows: fp64 operands follow ozaki_slices -- 6: six 8-bit digits for the
+// trailing updates of the Cholesky factorisation (K = panel width <= OZ8_MAX_K, where the int32 accumulators stay exact)
+// and seven 7-bit slices for every other product; 5, 7, 8: that many 7-bit slices.  The substitutions and the VFE
+// products keep the 7-bit format because their results are used directly and are held to the tile-GEMM path at 1e-8,
+// which the 8-bit bound (about 6x the 7-bit one) does not meet after C^-1 amplifies it.  fp32 operands take oz_S32
+// 7-bit slices.
+struct OzFmt { int S, bits; };
+template <typename T> static OzFmt slice_format(const agp_ctx* ctx, int64_t K, bool factor) {
+  if (!std::is_same<T, double>::value) return {ctx->oz_S32, 7};
+  if (ctx->oz_S == 6) return (factor && K <= OZ8_MAX_K) ? OzFmt{6, 8} : OzFmt{7, 7};
+  return {ctx->oz_S, 7};
 }
-static bool ensure_oz(agp_ctx* ctx, int64_t rows, int K, int S, cudaStream_t s) {
-  if (!ctx->oz.SL || ctx->oz.K != K || ctx->oz_rows < rows || ctx->oz.S != S) {
-    if (ctx->oz.SL) ozaki_ws_destroy(&ctx->oz, s);
-    if (ozaki_ws_create(&ctx->oz, rows, K, S, s) == 0) ctx->oz_rows = rows;
-    else { memset(&ctx->oz, 0, sizeof(ctx->oz)); ctx->oz_rows = 0; }
+// (re)size a cached slice workspace: rows x K bytes per slice in format f.  The requested format, not ozaki_slices, is
+// compared, so a long-K product that falls back to 7-bit slices keeps its workspace from call to call.
+static bool ensure_ws(OzakiWs& ws, int64_t& ws_rows, int64_t rows, int K, OzFmt f, cudaStream_t s) {
+  if (!ws.SL || ws.K != K || ws_rows < rows || ws.S != f.S || ws.bits != f.bits) {
+    if (ws.SL) ozaki_ws_destroy(&ws, s);
+    if (ozaki_ws_create(&ws, rows, K, f.S, s, f.bits) == 0) ws_rows = rows;
+    else { memset(&ws, 0, sizeof(ws)); ws_rows = 0; }
   }
-  return ctx->oz.SL != nullptr;
+  return ws.SL != nullptr;
+}
+// factor: the workspace serves the Cholesky's trailing updates (see slice_format)
+template <typename T> static bool ensure_oz2(agp_ctx* ctx, int64_t rows, int K, bool factor, cudaStream_t s) {  // second cached workspace (long-K products)
+  return ensure_ws(ctx->oz2, ctx->oz2_rows, rows, K, slice_format<T>(ctx, K, factor), s);
+}
+template <typename T> static bool ensure_oz(agp_ctx* ctx, int64_t rows, int K, bool factor, cudaStream_t s) {
+  return ensure_ws(ctx->oz, ctx->oz_rows, rows, K, slice_format<T>(ctx, K, factor), s);
 }
 
 // factor one outer panel in place: Lp points at its diagonal element; Gp inner 128-blocks; rows = rows from the
@@ -476,10 +487,10 @@ void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t ro
                       double* logdet_part, int* info) {
   cudaStream_t s = ctx->stream, s2 = ctx->stream2;
   const int nblk = (int)(n_pad / TILE);
-  const int fp64_mode = resolve_tensor_mode<T>(ctx, n_pad);  // 1: int8-sliced tensor-core trailing update (fp64: 7 slices, fp32: 4)
+  const int fp64_mode = resolve_tensor_mode<T>(ctx, n_pad);  // 1: int8-sliced tensor-core trailing update (fp64: slice_format, fp32: 4 slices)
   int G = resolve_G(ctx, n_pad);
   if (!std::is_same<T, double>::value && fp64_mode == 1 && ctx->cfg.tile_nb <= 0 && n_pad >= 4096) G = 4;  // 512-wide panels
-  const bool oz_ok = fp64_mode == 1 && nblk > 2 * G && ensure_oz(ctx, rows_total, G * TILE, slices_of<T>(ctx), s) &&
+  const bool oz_ok = fp64_mode == 1 && nblk > 2 * G && ensure_oz<T>(ctx, rows_total, G * TILE, true, s) &&
                      (std::is_same<T, double>::value || ctx->oz.bulk == 2);
   const bool la = ctx->cfg.lookahead != 0 && nblk > 2 * G;
   const bool la2 = la && ctx->cfg.lookahead >= 2;
@@ -575,7 +586,7 @@ bool forward_subst_multi_tc(agp_ctx* ctx, const T* L, int64_t lda, const T* Dinv
   const int nblk = (int)(n_pad / TILE);
   constexpr int is_f32 = std::is_same<T, double>::value ? 0 : 1;
   const int64_t a_rows = round_up(n_pad, TILE);
-  if (!ensure_oz(ctx, a_rows + ncols, (int)W, slices_of<T>(ctx), s) || ctx->oz.bulk != 2) return false;
+  if (!ensure_oz<T>(ctx, a_rows + ncols, (int)W, false, s) || ctx->oz.bulk != 2) return false;
   const OzakiWs& ws = ctx->oz;
   for (int ko = 0; ko < nblk; ko += GW) {
     const int k_end = (ko + GW < nblk) ? ko + GW : nblk;
@@ -655,7 +666,7 @@ bool backward_subst_multi_tc(agp_ctx* ctx, const T* L, int64_t lda, const T* Din
   const int nblk = (int)(n_pad / TILE);
   constexpr int is_f32 = std::is_same<T, double>::value ? 0 : 1;
   const int64_t a_rows = round_up(n_pad, TILE);
-  if (!ensure_oz(ctx, a_rows + ncols, (int)W, slices_of<T>(ctx), s) || ctx->oz.bulk != 2) return false;
+  if (!ensure_oz<T>(ctx, a_rows + ncols, (int)W, false, s) || ctx->oz.bulk != 2) return false;
   const OzakiWs& ws = ctx->oz;
   for (int ko = (nblk - 1) / GW * GW; ko >= 0; ko -= GW) {
     const int k_end = (ko + GW < nblk) ? ko + GW : nblk;
@@ -2606,7 +2617,7 @@ int vfe_core(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const agp_
     launch_scale_cols<T>(B, m_pad, m_pad, nc, isn + c0, s);
     forward_subst_multi<T>(ctx, Lz, lda, Dz, m_pad, B, m_pad, nc_pad);
     bool acc_done = false;
-    if (syrk_tc && nc_pad >= 1024 && ensure_oz2(ctx, m_pad, (int)nc_pad, slices_of<T>(ctx), s) && ctx->oz2.bulk == 2) {
+    if (syrk_tc && nc_pad >= 1024 && ensure_oz2<T>(ctx, m_pad, (int)nc_pad, false, s) && ctx->oz2.bulk == 2) {
       ozaki_prepare_ex(ctx->oz2, B, is_f32, 0, m_pad, m_pad, 0, s);
       acc_done = ozaki_update_ex(ctx->oz2, Lm, is_f32, lda, m_pad, m_pad, 0, 1.0, 0, 0, 0, 0, s) == 0;
     }
@@ -2764,7 +2775,7 @@ int vfe_grad_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
     // R is sliced once into rows [0, m_pad) of the workspace, each chunk of K_zx behind it
     constexpr int is_f32 = std::is_same<T, double>::value ? 0 : 1;
     bool g_tc = resolve_tensor_mode<T>(ctx, (int64_t)1 << 20) == 1 && mp >= 1024 && mp <= 32768 &&
-                ensure_oz2(ctx, mp + cap, (int)mp, slices_of<T>(ctx), s) && ctx->oz2.bulk == 2;
+                ensure_oz2<T>(ctx, mp + cap, (int)mp, false, s) && ctx->oz2.bulk == 2;
     if (g_tc) ozaki_prepare_ex(ctx->oz2, R, is_f32, 0, mp, mp, 0, s);
     CK(sc.alloc(&tmp, (size_t)(2 * nrb * cap + (int64_t)nsplit * D * mp) * sizeof(double)));
     double* qpart = (double*)tmp; double* upart = qpart + nrb * cap; double* zpart = upart + nrb * cap;
@@ -3125,12 +3136,7 @@ int fit_dist_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
   const OzakiWs* oz = nullptr;
   if constexpr (std::is_same<T, double>::value) {
     if (fp64_mode == 1 && nto > 2 && W % 64 == 0) {
-      if (!ctx->oz.SL || ctx->oz.K != W || ctx->oz_rows < lda || ctx->oz.S != ctx->oz_S) {
-        if (ctx->oz.SL) ozaki_ws_destroy(&ctx->oz, s);
-        if (ozaki_ws_create(&ctx->oz, lda, (int)W, ctx->oz_S, s) == 0) ctx->oz_rows = lda;
-        else { memset(&ctx->oz, 0, sizeof(ctx->oz)); ctx->oz_rows = 0; }
-      }
-      if (ctx->oz.SL) oz = &ctx->oz;
+      if (ensure_oz<T>(ctx, lda, (int)W, true, s)) oz = &ctx->oz;
     }
   }
   // schedule: 2 = pipelined (default for R > 1; see the loop below), 1 = round-1 owner-first experiment, 0 = plain look-ahead
@@ -3139,12 +3145,7 @@ int fit_dist_impl(agp_ctx* ctx, const agp_kernel* k, const agp_mean* mean, const
   const OzakiWs* oz_b = nullptr;  // second slice buffer (pipelined schedule only)
   if constexpr (std::is_same<T, double>::value) {
     if (dist_sched == 2 && oz) {
-      if (!ctx->oz2.SL || ctx->oz2.K != W || ctx->oz2_rows < lda || ctx->oz2.S != ctx->oz_S) {
-        if (ctx->oz2.SL) ozaki_ws_destroy(&ctx->oz2, s);
-        if (ozaki_ws_create(&ctx->oz2, lda, (int)W, ctx->oz_S, s) == 0) ctx->oz2_rows = lda;
-        else { memset(&ctx->oz2, 0, sizeof(ctx->oz2)); ctx->oz2_rows = 0; }
-      }
-      oz_b = ctx->oz2.SL ? &ctx->oz2 : nullptr;
+      oz_b = ensure_oz2<T>(ctx, lda, (int)W, true, s) ? &ctx->oz2 : nullptr;
       if (!oz_b) dist_sched = 0;
     }
   }
@@ -3489,8 +3490,8 @@ int32_t agp_init(agp_ctx** out, int32_t device, const agp_config* cfg) {
   ctx->cfg.lookahead = env_int("AGP_LOOKAHEAD", cfg ? ctx->cfg.lookahead : 2);  // 2: depth-2 look-ahead on the DMMA path
   ctx->cfg.use_graph = env_int("AGP_GRAPH", ctx->cfg.use_graph);
   ctx->profile = env_int("AGP_PROFILE", cfg ? cfg->profile_kernels : 0);
-  ctx->oz_S = env_int("AGP_OZAKI_S", (cfg && cfg->ozaki_slices) ? cfg->ozaki_slices : 7);
-  if (ctx->oz_S < 5 || ctx->oz_S > 8) ctx->oz_S = 7;
+  ctx->oz_S = env_int("AGP_OZAKI_S", (cfg && cfg->ozaki_slices) ? cfg->ozaki_slices : 6);
+  if (ctx->oz_S < 5 || ctx->oz_S > 8) ctx->oz_S = 6;
   ctx->oz_S32 = env_int("AGP_OZAKI_S32", 4);
   if (ctx->oz_S32 < 3 || ctx->oz_S32 > 5) ctx->oz_S32 = 4;
   if (cudaSetDevice(device) != cudaSuccess) { delete ctx; return AGP_ERR_CUDA; }
@@ -3804,6 +3805,43 @@ int32_t agp_debug_ozaki_syrk_map(agp_ctx* ctx, void* C_dev, int64_t ldc, const v
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { ctx->err = std::string("ozaki syrk (map): ") + cudaGetErrorString(e); return AGP_ERR_CUDA; }
   if (urc) { ctx->err = "ozaki syrk (map): strip table not supported"; return AGP_ERR_UNSUPPORTED; }
+  return AGP_OK;
+}
+
+int32_t agp_debug_ozaki8(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* A_dev, int32_t a_kmajor, int64_t lda,
+                         int64_t m_panel, const void* B_dev, int32_t b_kmajor, int64_t ldb, int64_t M, int64_t N, int32_t K,
+                         double sign, int64_t b_tile_stride, int64_t b_tile_width, int64_t b_off, int64_t a_off) {
+  if (!ctx || !C_dev || !A_dev) return AGP_ERR_INVALID;
+  if (N % 128 != 0 || N < 128 || M <= 0 || ldc < M) { ctx->err = "ozaki8: need 0 < M <= ldc, N a positive multiple of 128"; return AGP_ERR_INVALID; }
+  const int64_t m_pad = (M + 127) / 128 * 128;
+  if (B_dev) {
+    if (m_panel || b_tile_stride || b_tile_width || b_off || a_off) {
+      ctx->err = "ozaki8: a product with B takes no panel, column map or offsets";
+      return AGP_ERR_INVALID;
+    }
+  } else {
+    // rows and columns address the sliced panel in whole 128-row blocks: offsets and the column map must stay inside it
+    const int64_t bw = b_tile_width ? b_tile_width : 128;
+    const int64_t last_col_row = (b_tile_stride ? ((N - 1) / bw) * b_tile_stride + (N - 1) % bw : N - 1) + b_off;
+    if (m_panel <= 0 || a_off < 0 || b_off < 0 || a_off % 128 || b_off % 128 || b_tile_stride % 128 || bw % 128 ||
+        M + a_off > m_panel || last_col_row >= m_panel) {
+      ctx->err = "ozaki8: rows or columns outside the panel (offsets, stride and width in multiples of 128)";
+      return AGP_ERR_INVALID;
+    }
+  }
+  cudaSetDevice(ctx->device);
+  OzakiWs ws;
+  int rc = ozaki_ws_create(&ws, B_dev ? m_pad + N : m_panel, K, 6, ctx->stream, 8);
+  if (rc) { ctx->err = "ozaki_ws_create failed (code " + std::to_string(rc) + ")"; return rc == 1 ? AGP_ERR_INVALID : AGP_ERR_CUDA; }
+  ozaki_prepare_ex(ws, A_dev, 0, a_kmajor, lda, B_dev ? M : m_panel, 0, ctx->stream);
+  if (B_dev) ozaki_prepare_ex(ws, B_dev, 0, b_kmajor, ldb, N, m_pad, ctx->stream);
+  const int urc = ozaki_update_ex(ws, C_dev, 0, ldc, M, N, B_dev ? 1 : 0, sign, b_tile_stride, b_tile_width,
+                                  B_dev ? m_pad : b_off, a_off, ctx->stream);
+  ozaki_ws_destroy(&ws, ctx->stream);
+  cudaError_t e = cudaStreamSynchronize(ctx->stream);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) { ctx->err = std::string("ozaki8: ") + cudaGetErrorString(e); return AGP_ERR_CUDA; }
+  if (urc) { ctx->err = "ozaki8: K above 16384 or strip table not supported"; return AGP_ERR_UNSUPPORTED; }
   return AGP_OK;
 }
 

@@ -10,8 +10,9 @@
 // Splitting.  Row i of an operand is scaled by 2^-e_i (e_i: exponent of the row maximum) to |x| < 1 and cut into
 // S signed 7-bit slices  x = sum_s q_s 2^-(7s-1),  q_s in [-64, 64]  -- every step exact in fp64.
 // Then  a_i . b_j = 2^(e_i+e_j) sum_d 2^(-7d-5) ACC_d[i,j],  ACC_d = sum_{s+t=d+1} q_s . q_t  (int32, exact);
-// diagonals d > S are dropped (relative 2^(-7S)).  fp64: S = 7 (~2^-49 of the row scale; 5..8 selectable);
-// fp32: S = 4 (28 bits >= the 24-bit significand).
+// diagonals d > S are dropped (relative 2^(-7S)).  fp64: 5..8 selectable (S = 7: ~2^-49 of the row scale);
+// fp32: S = 4 (28 bits >= the 24-bit significand).  fp64 default: six balanced 8-bit digits instead (ozaki8_update_kernel,
+// see ozaki_slice_kernel and oz_combine), 21 MMAs per chunk for ~2^-43.4 of the row-scale products, K <= 16384.
 //
 // One kernel, ozaki_syrk_wgmma_kernel: persistent or bounded CTAs walking a list of 128 x BN output tiles; one producer
 // warp streams the slices with bulk copies, two consumer warpgroups (64 rows each) issue the MMAs and drain their own
@@ -98,10 +99,14 @@ __global__ void __launch_bounds__(256) ozaki_rowscale_kernel(const Tin* __restri
 
 // pre-pass 2: error-free slicing, 16 consecutive k per thread -> one 16-byte store per slice.  Rows land at
 // [dst_row0, dst_row0 + m_fill) of the slice buffer (dst_row0 a multiple of 128; rscale / rinv are already offset).
-template <int S, typename Tin>
+// BITS = 7: S balanced 7-bit digits peeled off in fp64.  BITS = 8 (S = 6): X = rint(y 2^46) as an int64, |X| <= 2^46, cut
+// into the balanced bytes q_5 .. q_1 in [-128, 127] (the low byte, sign-extended; X = (X - q) / 256 is exact) and the
+// leading digit q_0 = X, |q_0| <= 64; y = sum_s q_s 2^-(6+8s) to within 2^-47.
+template <int S, int BITS, typename Tin>
 __global__ void ozaki_slice_kernel(const Tin* __restrict__ P, int64_t lda, int64_t m, int64_t m_fill, int64_t m_alloc,
                                    int K, int kmajor, int64_t dst_row0, const double* __restrict__ rinv, int8_t* __restrict__ SL,
                                    int bulk) {
+  static_assert(BITS == 7 || (BITS == 8 && S == 6), "eight-bit digits come in six slices");
   const int64_t row = blockIdx.x * (int64_t)blockDim.x + threadIdx.x;
   const int k0 = blockIdx.y * 16;
   if (row >= m_fill) return;
@@ -116,15 +121,34 @@ __global__ void ozaki_slice_kernel(const Tin* __restrict__ P, int64_t lda, int64
   }
   double up = 64.0, dn = 1.0 / 64.0;  // 2^(7s-1), 2^-(7s-1)
   const int64_t drow = row + dst_row0;
+  int8_t q8[BITS == 8 ? S : 1][16];
+  if constexpr (BITS == 8) {
+#pragma unroll
+    for (int i = 0; i < 16; ++i) {
+      const double t = r[i] * 0x1p46;
+      long long X = (fabs(t) <= 0x1p46) ? __double2ll_rn(t) : 0;  // a non-finite entry (row scale NaN): no conversion
+#pragma unroll
+      for (int s = S - 1; s > 0; --s) {
+        const int q = (int)(int8_t)(X & 0xff);
+        q8[s][i] = (int8_t)q;
+        X = (X - q) >> 8;
+      }
+      q8[0][i] = (int8_t)X;
+    }
+  }
 #pragma unroll
   for (int s = 0; s < S; ++s) {
     union { int8_t b[16]; uint4 v; } pk;
 #pragma unroll
     for (int i = 0; i < 16; ++i) {
-      double q = rint(r[i] * up);
-      if (!(fabs(q) <= 64.0)) q = 0.0;  // only a non-finite entry gets here (its row scale is NaN): no int conversion of it
-      r[i] = fma(-q, dn, r[i]);
-      pk.b[i] = (int8_t)(int)q;
+      if constexpr (BITS == 8) {
+        pk.b[i] = q8[s][i];
+      } else {
+        double q = rint(r[i] * up);
+        if (!(fabs(q) <= 64.0)) q = 0.0;  // only a non-finite entry gets here (its row scale is NaN): no int conversion of it
+        r[i] = fma(-q, dn, r[i]);
+        pk.b[i] = (int8_t)(int)q;
+      }
     }
     if (bulk) {
       // no-swizzle K-major layout of the wgmma descriptors, written directly: chunk (slice, 128-row block, 32-byte
@@ -296,12 +320,18 @@ __device__ __forceinline__ double i64_to_f64_exact(long long x) {  // |x| < 2^51
 }
 // exact value of sum_d acc_d 128^(3-d) as two int64 words (hi: d = 0..3, lo: d = 4..S-1, scaled by 128^(S-4)), then ONE
 // rounding.  Accumulator block d of element i is acc[d * BN/2 + i].  PAIR32: adjacent accumulators are first combined in
-// int32 (valid for K <= 512).
-template <int S, int BN, bool PAIR32>
+// int32 (valid for K <= 512).  BITS = 8 (six 8-bit digits): h = sum_{d<3} ACC_d 256^(2-d), l = sum_{d>=3} ACC_d 256^(5-d),
+// v = h + 2^-24 l = 2^16 sum_d ACC_d 256^-d; |h|, |l| < 2^47 for K <= 16384.
+template <int S, int BITS, int BN, bool PAIR32>
 __device__ __forceinline__ double oz_combine(const uint32_t* acc, int i) {
   auto r = [&](int d) { return (int)acc[d * (BN / 2) + i]; };
   long long h = 0, l = 0;
-  if constexpr (S <= 4) {  // fp32 operands (3 or 4 slices): everything fits one word, the conversion is the only rounding
+  if constexpr (BITS == 8) {
+    static_assert(S == 6 && !PAIR32, "eight-bit digits: six slices, int64 words only");
+    h = ((long long)r(0) * 256 + r(1)) * 256 + r(2);
+    l = ((long long)r(3) * 256 + r(4)) * 256 + r(5);
+    return fma(i64_to_f64_exact(l), 1.0 / 16777216.0, i64_to_f64_exact(h));
+  } else if constexpr (S <= 4) {  // fp32 operands (3 or 4 slices): everything fits one word, the conversion is the only rounding
     h = r(0);
 #pragma unroll
     for (int d = 1; d < S; ++d) h = h * 128 + r(d);
@@ -350,9 +380,10 @@ __device__ __forceinline__ void oz_chunk(uint32_t* acc, uint32_t (&af)[S][4], ui
 }
 
 // the drain of one consumer thread: rows r0, r0 + 8 of the tile and columns 8j + 2(lane & 3) + {0, 1} of every
-// accumulator block; C += sign * (2^e_i 2^e_j 2^-33) * v with rs[h] = sign 2^e_i 2^-33, streamed (.cs) so the int8
-// slices stay resident in L2.  STAGED: a full tile whose old C is in the staged block; otherwise guarded global loads.
-template <int S, int BN, bool PAIR32, bool STAGED, typename CT>
+// accumulator block; C += sign * (2^e_i 2^e_j 2^-33) * v with rs[h] = sign 2^e_i 2^-33 (2^-28 for 8-bit digits), streamed
+// (.cs) so the int8 slices stay resident in L2.  STAGED: a full tile whose old C is in the staged block; otherwise guarded
+// global loads.
+template <int S, int BITS, int BN, bool PAIR32, bool STAGED, typename CT>
 __device__ __forceinline__ void oz_drain(const OzTileArgs& a, const uint32_t* acc, const CT* cbuf, int bi, int bj, int64_t brow,
                                          int r0, const double* rs) {
   constexpr int C_LD = OzCfg<S, CT>::C_LD;
@@ -373,14 +404,15 @@ __device__ __forceinline__ void oz_drain(const OzTileArgs& a, const uint32_t* ac
     for (int i = i0; i < i0 + 8; ++i) {
       const int c = 8 * (i >> 2) + cq + (i & 1), h = (i >> 1) & 1;
       const int64_t row = m0 + 8 * h, col = (int64_t)bj * BN + c;
-      const double v = oz_combine<S, BN, PAIR32>(acc, i);
+      const double v = oz_combine<S, BITS, BN, PAIR32>(acc, i);
       if (STAGED || (row < a.M && col < a.N)) st_cs(C + row + col * a.ldc, fma(v, rs[h] * a.rscale[brow + c], cv[i - i0]));
     }
   }
 }
 
-template <int S, typename CT>
-__global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileArgs a, int64_t ntiles, int nbi, int nbj, int tpc) {
+// the body of the update kernels; BITS is the digit width of the slices (7 or 8), which only the drain sees
+template <int S, int BITS, typename CT>
+__device__ __forceinline__ void oz_syrk_body(const OzTileArgs& a, int64_t ntiles, int nbi, int nbj, int tpc) {
   // tpc = 0: persistent, CTA b walks slots b, b + grid, ...   tpc > 0: BOUNDED CTAs -- CTA b owns the tpc consecutive slots
   // [b * tpc, (b + 1) * tpc) and exits; the grid is ceil(ntiles / tpc).  Bounded CTAs hand their SM back every ~0.1 ms, so
   // kernels of a higher-priority stream (the panel chain, the NCCL broadcast) are scheduled between them instead of
@@ -493,16 +525,18 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileA
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int64_t row = (int64_t)bi * OZ_BM + r0 + 8 * h;
-        rs[h] = row < a.M ? a.sign * a.rscale[row + a.a_off] * (1.0 / 8589934592.0) : 0.0;  // +-2^e_i * 2^-12 * 128^-3
+        // 7 bits: +-2^e_i * 2^-12 * 128^-3;  8 bits: +-2^e_i * 2^-12 * 2^-16 (v carries 2^16 sum_d ACC_d 256^-d)
+        constexpr double SCALE = (BITS == 8) ? 1.0 / 268435456.0 : 1.0 / 8589934592.0;
+        rs[h] = row < a.M ? a.sign * a.rscale[row + a.a_off] * SCALE : 0.0;
       }
       const bool staged = oz_c_staged<BN>(a, bi, bj);
       if (staged) mbar_wait(&c_full, cn & 1);
-      if (a.epi == 1) {
-        if (staged) oz_drain<S, BN, true, true>(a, acc, cbuf, bi, bj, brow, r0, rs);
-        else oz_drain<S, BN, true, false>(a, acc, cbuf, bi, bj, brow, r0, rs);
+      if (BITS == 7 && a.epi == 1) {
+        if (staged) oz_drain<S, BITS, BN, BITS == 7, true>(a, acc, cbuf, bi, bj, brow, r0, rs);
+        else oz_drain<S, BITS, BN, BITS == 7, false>(a, acc, cbuf, bi, bj, brow, r0, rs);
       } else {
-        if (staged) oz_drain<S, BN, false, true>(a, acc, cbuf, bi, bj, brow, r0, rs);
-        else oz_drain<S, BN, false, false>(a, acc, cbuf, bi, bj, brow, r0, rs);
+        if (staged) oz_drain<S, BITS, BN, false, true>(a, acc, cbuf, bi, bj, brow, r0, rs);
+        else oz_drain<S, BITS, BN, false, false>(a, acc, cbuf, bi, bj, brow, r0, rs);
       }
       if (staged) {  // this warp has read its part of the staged block
         __syncwarp();
@@ -513,20 +547,41 @@ __global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileA
   }
 }
 
+// seven-bit slices: fp64 C with 4..8 slices, fp32 C with 3..5
+template <int S, typename CT>
+__global__ void __launch_bounds__(OZ_THREADS, 1) ozaki_syrk_wgmma_kernel(OzTileArgs a, int64_t ntiles, int nbi, int nbj, int tpc) {
+  oz_syrk_body<S, 7, CT>(a, ntiles, nbi, nbj, tpc);
+}
+// six eight-bit slices, fp64 C
+__global__ void __launch_bounds__(OZ_THREADS, 1) ozaki8_update_kernel(OzTileArgs a, int64_t ntiles, int nbi, int nbj, int tpc) {
+  oz_syrk_body<6, 8, double>(a, ntiles, nbi, nbj, tpc);
+}
+
+template <int S, int BITS, typename CT>
+struct OzKernel {
+  static_assert(BITS == 7, "eight-bit digits: six slices and fp64 C only");
+  static constexpr auto fn = ozaki_syrk_wgmma_kernel<S, CT>;
+};
+template <>
+struct OzKernel<6, 8, double> {
+  static constexpr auto fn = ozaki8_update_kernel;
+};
+
 // C += sign * P_A P_B' on the slices in ws.  full = 0: lower tiles only; returns 1 if the shape needs a longer strip
 // table than the workspace holds.
-template <int S, typename CT>
+template <int S, int BITS, typename CT>
 int launch_syrk_wgmma(const OzakiWs& ws, void* C, int64_t ldc, int64_t M, int64_t N, int64_t b_tile_stride,
                       int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s, int full, double sign) {
   using Cfg = OzCfg<S, CT>;
   constexpr int BN = Cfg::BN, R = OZ_BM / BN;
+  constexpr auto kernel = OzKernel<S, BITS, CT>::fn;
   static uint64_t configured = 0;  // per-device bit: the attribute is per device (one ctx per GPU in one process)
   static int nsm = 0;
   if (agp_first_use_on_device(&configured)) {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
-    cudaFuncSetAttribute(ozaki_syrk_wgmma_kernel<S, CT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
+    cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
   }
   OzTileArgs a{};
   a.C = C; a.ldc = ldc; a.M = M; a.N = N; a.K = ws.K; a.rscale = ws.rscale;
@@ -539,7 +594,7 @@ int launch_syrk_wgmma(const OzakiWs& ws, void* C, int64_t ldc, int64_t M, int64_
     // AGP_OZAKI_EPI=0 restores the plain int64 drain
     const char* e = getenv("AGP_OZAKI_EPI");
     a.epi = (e && atoi(e) == 0) ? 0 : 1;
-    if (ws.K > 512) a.epi = 0;  // the int32 pair bound needs K <= 512
+    if (ws.K > 512 || BITS == 8) a.epi = 0;  // the int32 pair bound needs K <= 512 (at 8 bits 256 ACC wraps from K = 512)
   }
   const int nbi = (int)((M + OZ_BM - 1) / OZ_BM), nbj = (int)((N + BN - 1) / BN);
   int64_t ntiles = 0;
@@ -576,18 +631,18 @@ int launch_syrk_wgmma(const OzakiWs& ws, void* C, int64_t ldc, int64_t M, int64_
   int64_t grid = cap < ntiles ? cap : ntiles;
   const int tpc = ws.chunk_tiles;
   if (tpc > 0) grid = (ntiles + tpc - 1) / tpc;
-  ozaki_syrk_wgmma_kernel<S, CT><<<(unsigned)grid, OZ_THREADS, Cfg::SMEM, s>>>(a, ntiles, nbi, nbj, tpc);
+  kernel<<<(unsigned)grid, OZ_THREADS, Cfg::SMEM, s>>>(a, ntiles, nbi, nbj, tpc);
   agp_count_launch();
   return 0;
 }
 
 }  // namespace
 
-int ozaki_ws_create(OzakiWs* ws, int64_t max_rows, int K, int S, cudaStream_t s) {
+int ozaki_ws_create(OzakiWs* ws, int64_t max_rows, int K, int S, cudaStream_t s, int bits) {
   memset(ws, 0, sizeof(*ws));
-  if (S < 3 || S > 8 || K % 64 != 0) return 1;
+  if (S < 3 || S > 8 || K % 64 != 0 || (bits != 7 && bits != 8) || (bits == 8 && S != 6)) return 1;
   ws->m_alloc = (max_rows + 127) / 128 * 128;
-  ws->K = K; ws->S = S;
+  ws->K = K; ws->S = S; ws->bits = bits;
   if (cudaMallocAsync((void**)&ws->SL, (size_t)S * ws->m_alloc * K, s) != cudaSuccess) return 3;
   if (cudaMallocAsync((void**)&ws->rscale, (size_t)ws->m_alloc * 2 * sizeof(double), s) != cudaSuccess) return 3;
   ws->rinv = ws->rscale + ws->m_alloc;
@@ -615,14 +670,18 @@ static void prepare_t(const OzakiWs& ws, const Tin* P, int kmajor, int64_t lda, 
   agp_count_launch();
   const int64_t m_used = (m + 127) / 128 * 128;  // zero-fill up to the tile edge
   dim3 grid((unsigned)((m_used + 127) / 128), (unsigned)(ws.K / 16));
-#define AGP_SLICE(SS) ozaki_slice_kernel<SS, Tin><<<grid, 128, 0, s>>>(P, lda, m, m_used, ws.m_alloc, ws.K, kmajor, dst_row0, ri, ws.SL, ws.bulk)
-  switch (ws.S) {
-    case 3: AGP_SLICE(3); break;
-    case 4: AGP_SLICE(4); break;
-    case 5: AGP_SLICE(5); break;
-    case 6: AGP_SLICE(6); break;
-    case 7: AGP_SLICE(7); break;
-    default: AGP_SLICE(8); break;
+#define AGP_SLICE(SS, BB) ozaki_slice_kernel<SS, BB, Tin><<<grid, 128, 0, s>>>(P, lda, m, m_used, ws.m_alloc, ws.K, kmajor, dst_row0, ri, ws.SL, ws.bulk)
+  if (ws.bits == 8) {
+    AGP_SLICE(6, 8);
+  } else {
+    switch (ws.S) {
+      case 3: AGP_SLICE(3, 7); break;
+      case 4: AGP_SLICE(4, 7); break;
+      case 5: AGP_SLICE(5, 7); break;
+      case 6: AGP_SLICE(6, 7); break;
+      case 7: AGP_SLICE(7, 7); break;
+      default: AGP_SLICE(8, 7); break;
+    }
   }
 #undef AGP_SLICE
   agp_count_launch();
@@ -645,7 +704,11 @@ int ozaki_update_ex(const OzakiWs& ws, void* C, int c_is_float, int64_t ldc, int
   if (M <= 0 || N <= 0) return 0;
   if (ws.bulk != 2 || N % 128 != 0) return 1;
   if (ws.K > 32768) return 1;  // int32 accumulators ((d+1) K 64^2 < 2^31) and the 2^51 range of the exact int64 -> fp64 drain
-#define AGP_UPD(SS, CTT) return launch_syrk_wgmma<SS, CTT>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, sign)
+#define AGP_UPD(SS, CTT) return launch_syrk_wgmma<SS, 7, CTT>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, sign)
+  if (ws.bits == 8) {
+    if (c_is_float || ws.K > OZ8_MAX_K) return 1;
+    return launch_syrk_wgmma<6, 8, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, sign);
+  }
   if (c_is_float) {
     switch (ws.S) {
       case 3: AGP_UPD(3, float);
@@ -670,11 +733,15 @@ int ozaki_syrk(const OzakiWs& ws, double* C, int64_t ldc, int64_t M, int64_t N, 
                int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s) {
   if (M <= 0 || N <= 0) return 0;
   const int full = lower_only ? 0 : 1;
+  if (ws.bits == 8) {
+    if (ws.K > OZ8_MAX_K) return 1;
+    return launch_syrk_wgmma<6, 8, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+  }
   switch (ws.S) {
-    case 5: return launch_syrk_wgmma<5, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
-    case 6: return launch_syrk_wgmma<6, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
-    case 7: return launch_syrk_wgmma<7, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
-    case 8: return launch_syrk_wgmma<8, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    case 5: return launch_syrk_wgmma<5, 7, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    case 6: return launch_syrk_wgmma<6, 7, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    case 7: return launch_syrk_wgmma<7, 7, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
+    case 8: return launch_syrk_wgmma<8, 7, double>(ws, C, ldc, M, N, b_tile_stride, b_tile_width, b_off, a_off, s, full, -1.0);
     default: return 1;  // fp64 C is instantiated for 5..8 slices only (a 3- or 4-slice workspace is for fp32 panels)
   }
 }

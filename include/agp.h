@@ -114,7 +114,10 @@ typedef struct {
   int32_t lookahead;     /* 0 off, 1: overlap the next panel with the bulk of the trailing update, 2 (default): additionally
                             split the bulk so that the chain waits only for the panel-after-next block (DMMA path) */
   int32_t use_graph;     /* reserved */
-  int32_t ozaki_slices;  /* 5..8 seven-bit slices of the int8 fp64 path; 0 -> 7 (~2^-49 of the row scale) */
+  int32_t ozaki_slices;  /* slices of the int8 fp64 path; 0 -> 6.  6: six balanced 8-bit digits (21 int8 MMAs per fp64 MAC,
+                            error <= 2^-43.4 2^(e_i+e_j) K) in the Cholesky's trailing updates, seven 7-bit slices in
+                            the substitutions and VFE products; 5, 7, 8: that many 7-bit slices everywhere
+                            ((S + 1.06) 2^-7S 2^(e_i+e_j) K; 7 -> 2^-46) */
   int32_t profile_kernels; /* 1: CUDA events around every trailing-update launch (agp_last_timings[7]); default 0 */
   int32_t reserved[9];
 } agp_config; /* NULL -> defaults; env AGP_NB, AGP_FP64_MODE, AGP_FP32_MODE, AGP_LOOKAHEAD, AGP_OZAKI_S, AGP_OZAKI_S32 override at agp_init */
@@ -483,6 +486,16 @@ int32_t agp_debug_ozaki_gemm(agp_ctx* ctx, void* C_dev, int32_t c_is_float, int6
 int32_t agp_debug_ozaki_syrk_map(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* P_dev, int64_t lda, int64_t m_panel,
                                  int64_t M, int64_t N, int32_t K, int32_t S, int64_t b_tile_stride, int64_t b_tile_width,
                                  int64_t b_off, int64_t a_off);
+/* the six-slice eight-bit format of the fp64 path (ozaki_slices = 6), K % 64 == 0 and K <= 16384 (else
+ * AGP_ERR_UNSUPPORTED), fp64 operands and C, C (M x N, N % 128 == 0) += sign * A B':
+ *  - B_dev != NULL: rectangular product of A (M rows) and B (N rows), each row-contiguous or k-major (*_kmajor);
+ *    m_panel, b_tile_stride, b_tile_width, b_off and a_off must be 0;
+ *  - B_dev == NULL: A is a panel of m_panel rows, lower tiles only; row r of C pairs with panel row r + a_off, column n
+ *    with panel row (n / b_tile_width) * b_tile_stride + n % b_tile_width + b_off (stride 0: n + b_off), all in
+ *    multiples of 128 -- the closed-form walk when stride == 0 and a_off == b_off, the strip table otherwise. */
+int32_t agp_debug_ozaki8(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* A_dev, int32_t a_kmajor, int64_t lda,
+                         int64_t m_panel, const void* B_dev, int32_t b_kmajor, int64_t ldb, int64_t M, int64_t N, int32_t K,
+                         double sign, int64_t b_tile_stride, int64_t b_tile_width, int64_t b_off, int64_t a_off);
 
 /* ---- host-only helpers of the 2D block-cyclic tile map (no GPU needed; used by the CPU
  * world_size-2 tests): owner rank of tile (i,j) on a P x Q grid and local tile counts. */
