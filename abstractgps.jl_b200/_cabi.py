@@ -84,6 +84,8 @@ SIGNATURES = {
                                               C.POINTER(C.c_double), _P, _P, _P, _P, _P, _P, _P, _P]),
     "agp_post_rand_grad": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _M, _N, _P, C.c_int32, _P, C.POINTER(C.c_double), _P,
                                        _P, _P, _P, _P, _P, _P, _P]),
+    "agp_post_mean_var_grad": (C.c_int32, [_P, C.c_int32, _P, C.c_int64, _P, _P, C.POINTER(C.c_double), _P, _P, _P, _P,
+                                           _P]),
     "agp_post_grad_len": (C.c_int64, [_P]),
     "agp_post_solve_lower": (C.c_int32, [_P, _P, C.c_int64, _P]),
     "agp_post_factor_export": (C.c_int32, [_P, _P]),

@@ -1121,6 +1121,61 @@ def posterior_rand_grad(fx: FiniteGP, Z, out_bar, inputs=False):
     return (out[:, 0].copy() if ndim == 1 else out), res
 
 
+def posterior_mean_var_grad(fx: FiniteGP, mean_bar, var_bar, inputs=False, training=True):
+    """((mean, var), gradient dict) of mean_and_var(fx) for fx = p(x*, s2*) over an exact posterior p = posterior(fx0, y),
+    pulled back from the cotangents mean_bar and var_bar (M values each; None means zeros): what Zygote returns through
+    mean_and_var over a posterior, for analytic acquisition functions (expected improvement, probability of improvement,
+    UCB) and losses on predicted means.  (mean, var) is agp_post_mean_var's on p's handle; the dict comes from one
+    agp_post_mean_var_grad call.  Its keys are those of posterior_rand_grad without "Z": the kernel keys, the training
+    side "noise", "mean_c" | "mean_v" and "y", the test side "noise_s" (var_bar per point, or its sum for a scalar s2*)
+    and "mean_s_v" (mean_bar, CustomMean only); a ConstMean's "mean_c" counts both sides.  inputs=True also returns "x"
+    and "xs", shaped like the containers the points came in.  training=False passes NULL for every training-side output
+    and returns only the test side ("noise_s", "mean_s_v" and, with inputs=True, "xs"): the call an optimiser over x*
+    makes, which does no N x N work.  A CustomMean is treated as a constant of the inputs.  Only a posterior straight
+    from posterior(fx0, y) is supported (not a sequentially conditioned one)."""
+    p = fx.f
+    if not isinstance(p, PosteriorGP) or getattr(p, "fx", None) is None:
+        raise AGPError(cabi.AGP_ERR_UNSUPPORTED, "the gradient of mean_and_var over a posterior needs a FiniteGP over "
+                       "posterior(fx, y), not over %s" % type(p).__name__)
+    eng = engine()
+    p, dt, pts, ms, ns, keep = _post_args(fx)
+    fx0 = p.fx
+    N, M, D = p.data.x.n, pts.n, pts.D
+
+    def cot(a, name):
+        if a is None:
+            return None
+        v = np.ascontiguousarray(np.asarray(a, dtype=dt).ravel())
+        if v.shape[0] != M:
+            raise DimensionMismatch("%s has %d entries, length(fx) = %d" % (name, v.shape[0], M))
+        return v
+    mb, vb = cot(mean_bar, "mean_bar"), cot(var_bar, "var_bar")
+    mv = _post_call(p, pts, fx.s2)
+    f = p.prior
+    k = f.kernel
+    g, flat = _grad_buffer(k, D, p.data.C.h) if training else (None, None)
+    nd = np.empty(N, dtype=dt) if training and np.ndim(fx0.s2) != 0 else None
+    md = np.empty(N, dtype=dt) if training and isinstance(f.mean, CustomMean) else None
+    yb = np.empty(N, dtype=dt) if training else None
+    xg = _points_grad(fx0.x_kind, N, D, dt) if inputs and training else None  # the points go in point-major
+    xsg = _points_grad(fx.x_kind, M, D, dt) if inputs else None
+    eng.check(eng.L.agp_post_mean_var_grad(p.data.C.h, cabi.AGP_POINT_MAJOR, cabi.ptr(pts.a), M, cabi.ptr(mb),
+                                           cabi.ptr(vb), None if g is None else g.ctypes.data_as(C.POINTER(C.c_double)),
+                                           cabi.ptr(nd), cabi.ptr(md), cabi.ptr(yb), cabi.ptr(xg), cabi.ptr(xsg)))
+    res = _grad_result(g, flat, k, D, f.mean, nd, md) if training else {}
+    if training:
+        res["y"] = yb
+    vb64 = np.zeros(M) if vb is None else vb.astype(np.float64)
+    res["noise_s"] = vb64 if np.ndim(fx.s2) != 0 else float(np.sum(vb64))
+    if isinstance(f.mean, CustomMean):
+        res["mean_s_v"] = np.zeros(M) if mb is None else mb.astype(np.float64)
+    if inputs:
+        if training:
+            res["x"] = xg
+        res["xs"] = xsg
+    return mv, res
+
+
 def _post_call(p: PosteriorGP, pts: _Points, s2, want_var=True, want_cov=False):
     eng = engine()
     dt = p.data.C.dtype

@@ -2453,6 +2453,114 @@ int post_rand_grad_impl(agp_post* p, int layout, const void* Xs, int64_t M, cons
   return AGP_OK;
 }
 
+// ---- pullback of mean_and_var(posterior(fx, y)(x*)) on a handle from agp_fit (agp.h agp_post_mean_var_grad).  With
+// A = L^-1 K_xs and P = C^-1 K_xs = L^-T A (forward_subst_multi, then backward_subst_multi: N^2 M, no L^-1 or C^-1), the
+// cotangents mbar of the means and vbar of the variances are the held-out gradient's mubar and Sigmabar = diag(vbar):
+//   Kbar_sx[j, n] = mbar_j alpha_n - 2 vbar_j P[n, j],  beta = P mbar,  Cbar = P diag(vbar) P' - 1/2 (beta alpha' + alpha beta').
+// mu*, Sigma and its factor never enter: the call takes neither the test mean nor the test noise.
+//   - x* side: xs_grad_out always comes from launch_cross_grad_x, one pass over the N x M pairs with Kbar_sx formed from P
+//     on the fly (post_xs_grad.cu), whatever else is asked for.
+//   - training side: the kernel, noise and x outputs run post_pred_tail unchanged with Ws = -2 diag(vbar) and mubar = mbar
+//     (its test-side outputs NULL); y_bar_out and mean_diag_out alone need only beta, one GEMV, and skip the stacked pass.
+// Without a kernel, noise or x output the call allocates A and P (P = A in place: about NM elements) and the cross
+// pass's O((N + M) D); the training side adds the tail's m_pad (m_pad + 16) Ws and (N + M)^2 stacked W.
+template <typename T>
+int post_mean_var_grad_impl(agp_post* p, int layout, const void* Xs, int64_t M, const void* mean_bar, const void* var_bar,
+                            double* grad_out, void* noise_diag_out, void* mean_diag_out, void* y_bar_out, void* x_grad_out,
+                            void* xs_grad_out) {
+  agp_ctx* ctx = p->ctx;
+  if (!Xs) { ctx->err = "Xs is NULL"; return AGP_ERR_INVALID; }
+  if (M <= 0) { ctx->err = "M must be positive"; return AGP_ERR_DIM_MISMATCH; }
+  int rc = logpdf_grad_prelude<T>(p, layout);
+  if (rc) return rc;
+  cudaStream_t s = ctx->stream;
+  const int64_t N = p->n, n_pad = p->n_pad, m_pad = round_up(M, TILE);
+  const int D = p->D;
+  constexpr int64_t XK = POST_XK;
+  const bool want_red = grad_out || noise_diag_out || x_grad_out;
+  const bool want_beta = want_red || mean_diag_out || y_bar_out;
+  if (!want_beta && !xs_grad_out) return AGP_OK;
+  Scratch sc(ctx);
+  void* tmp = nullptr;
+  auto drop = [&](void* q) { sc.release(q); cudaFreeAsync(q, s); };
+
+  // the cotangents on the device, m_pad values each with zero padding (NULL: zeros)
+  CK(sc.alloc(&tmp, (size_t)m_pad * 2 * sizeof(T)));
+  T* mbar = (T*)tmp;
+  T* vbar = mbar + m_pad;
+  CK(cudaMemsetAsync(mbar, 0, (size_t)m_pad * 2 * sizeof(T), s));
+  const cudaMemcpyKind kin = ctx->memspace == AGP_MEM_DEVICE ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice;
+  if (mean_bar) CK(cudaMemcpyAsync(mbar, mean_bar, (size_t)M * sizeof(T), kin, s));
+  if (var_bar) CK(cudaMemcpyAsync(vbar, var_bar, (size_t)M * sizeof(T), kin, s));
+
+  // ---- forward: A = L^-1 K_xs, then P = L^-T A (with room for the tail's alpha column when the tail runs)
+  T *Xst = nullptr, *A = nullptr;
+  rc = post_cross<T>(p, sc, layout, Xs, M, m_pad, &Xst, &A);
+  if (rc) return rc;
+  forward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, A, n_pad, m_pad);
+  T* P = A;
+  if (want_red) {
+    CK(sc.alloc(&tmp, (size_t)n_pad * (m_pad + XK) * sizeof(T)));
+    P = (T*)tmp;
+    CK(cudaMemcpyAsync(P, A, (size_t)n_pad * m_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    drop(A);
+  }
+  backward_subst_multi<T>(ctx, (const T*)p->L, p->lda, (const T*)p->Dinv, n_pad, P, n_pad, m_pad);
+
+  // ---- x* side: one pass over the N x M pairs
+  if (xs_grad_out) {
+    const CompositeDesc one = single_kernel_desc(p->k.family, p->k.variance, p->k.linear_c);
+    const CompositeDesc* cd = &one;
+    double mult = 1.0;
+    const T* ard = nullptr;
+    if (p->comp) {
+      cd = &p->comp->desc;
+    } else {
+      if (p->k.transform == AGP_T_SCALE) mult = p->k.scale;
+      else if (p->k.transform == AGP_T_ARD) ard = (const T*)p->ard;
+    }
+    CK(sc.alloc(&tmp, (size_t)cross_grad_x_part_len(M, N, D, cd->nacc) * sizeof(double)));
+    double* part = (double*)tmp;
+    CK(sc.alloc(&tmp, (size_t)M * D * sizeof(T)));
+    T* xsg = (T*)tmp;
+    launch_cross_grad_x<T>(Xst, M, (const T*)p->Xt, N, D, P, n_pad, (const T*)p->alpha, mbar, vbar, *cd, mult, ard, layout,
+                           part, xsg, s);
+    rc = download<T>(ctx, xs_grad_out, xsg, (size_t)M * D, false);
+    if (rc) return rc;
+  }
+
+  // ---- training side
+  if (want_red) {  // Ws = -2 diag(vbar) and mubar = mbar in column m_pad, then post_pred_tail
+    CK(sc.alloc(&tmp, (size_t)m_pad * (m_pad + XK) * sizeof(T)));
+    T* Ws = (T*)tmp;
+    CK(cudaMemsetAsync(Ws, 0, (size_t)m_pad * (m_pad + XK) * sizeof(T), s));
+    CK(cudaMemcpy2DAsync(Ws, (size_t)(m_pad + 1) * sizeof(T), vbar, sizeof(T), sizeof(T), (size_t)M,
+                         cudaMemcpyDeviceToDevice, s));  // the diagonal
+    launch_scale<T>(Ws, m_pad * m_pad, -2.0, s);
+    CK(cudaMemcpyAsync(Ws + m_pad * m_pad, mbar, (size_t)M * sizeof(T), cudaMemcpyDeviceToDevice, s));
+    rc = post_pred_tail<T>(p, sc, layout, Xst, M, Ws, P, true, grad_out, noise_diag_out, mean_diag_out, y_bar_out,
+                           x_grad_out, nullptr, nullptr);
+    if (rc) return rc;
+  } else if (want_beta) {  // ybar = beta = P mbar, mbar at x = -beta (the tail's GEMV)
+    CK(sc.alloc(&tmp, (size_t)n_pad * 2 * sizeof(T)));
+    T* beta = (T*)tmp;
+    T* nbeta = beta + n_pad;
+    CK(cudaMemsetAsync(beta, 0, (size_t)n_pad * 2 * sizeof(T), s));
+    launch_gemv_n_acc<T>(P, n_pad, N, M, mbar, beta, s);
+    rc = download<T>(ctx, y_bar_out, beta, (size_t)N, false);
+    if (rc) return rc;
+    if (mean_diag_out) {
+      CK(cudaMemcpyAsync(nbeta, beta, (size_t)n_pad * sizeof(T), cudaMemcpyDeviceToDevice, s));
+      launch_scale<T>(nbeta, n_pad, -1.0, s);
+      rc = download<T>(ctx, mean_diag_out, nbeta, (size_t)N, false);
+      if (rc) return rc;
+    }
+  }
+  CK(cudaStreamSynchronize(s));
+  CK(cudaGetLastError());
+  return AGP_OK;
+}
+
 template <typename T>
 int gram_impl(agp_ctx* ctx, const agp_kernel* k, int layout, const void* X, int64_t N, int D, const void* Z,
               int64_t M, const agp_noise* noise, void* K_out) {
@@ -3671,6 +3779,17 @@ int32_t agp_post_rand_grad(agp_post* p, int32_t layout, const void* Xs, int64_t 
                   post_rand_grad_impl<double>(p, layout, Xs, M, mean_s, noise_s, Z, S, out_bar, grad_out, noise_diag_out,
                                               mean_diag_out, y_bar_out, x_grad_out, noise_s_diag_out, mean_s_diag_out,
                                               z_bar_out, xs_grad_out));
+}
+
+int32_t agp_post_mean_var_grad(agp_post* p, int32_t layout, const void* Xs, int64_t M, const void* mean_bar,
+                               const void* var_bar, double* grad_out, void* noise_diag_out, void* mean_diag_out,
+                               void* y_bar_out, void* x_grad_out, void* xs_grad_out) {
+  if (!p) return AGP_ERR_INVALID;
+  return DISPATCH(p->dtype,
+                  post_mean_var_grad_impl<float>(p, layout, Xs, M, mean_bar, var_bar, grad_out, noise_diag_out,
+                                                 mean_diag_out, y_bar_out, x_grad_out, xs_grad_out),
+                  post_mean_var_grad_impl<double>(p, layout, Xs, M, mean_bar, var_bar, grad_out, noise_diag_out,
+                                                  mean_diag_out, y_bar_out, x_grad_out, xs_grad_out));
 }
 
 int32_t agp_post_solve_lower(agp_post* p, const void* B, int64_t nrhs, void* V_out) {

@@ -167,6 +167,14 @@ int64_t grad_x_part_len(int64_t n, int D, int nacc);
 template <typename T> void launch_grad_x(const T* X, int D, int64_t n, const T* Cinv, int64_t ldc, const T* alpha,
                                          const CompositeDesc& cd, double mult, const T* ard, int layout, double* part,
                                          T* out, cudaStream_t s);
+// test-point gradient of mean_and_var over a posterior (post_xs_grad.cu): out (m x D values in `layout`) = mult * chain_d *
+// (sum_n Kbar_sx[j, n] d1k(x*_j, x_n)_d + 2 vbar_j d1k(x*_j, x*_j)_d), Kbar_sx[j, n] = mbar_j alpha_n - 2 vbar_j P[n + j*ldp],
+// over the descriptor cd on the test points Xs (m x D) and the training points X (n x D), both point-major; mbar and vbar
+// hold m values.  part: workspace of cross_grad_x_part_len(m, n, D, cd.nacc) doubles (zeroed inside)
+int64_t cross_grad_x_part_len(int64_t m, int64_t n, int D, int nacc);
+template <typename T> void launch_cross_grad_x(const T* Xs, int64_t m, const T* X, int64_t n, int D, const T* P, int64_t ldp,
+                                               const T* alpha, const T* mbar, const T* vbar, const CompositeDesc& cd,
+                                               double mult, const T* ard, int layout, double* part, T* out, cudaStream_t s);
 // gradient of the VFE objectives (vfe_grad.cu).  H = c I - Lam^-1 - m_e m_e', E = c D - I + Lam^-1 + m_e m_e' (m_pad x m_pad,
 // full, 0 outside M x M) from Lam^-1 (full), D = Lam - I (lower storage) and m_e
 template <typename T> void launch_vfe_hz(const T* Laminv, const T* Dl, int64_t ldd, const T* me, int64_t M, int64_t m_pad,

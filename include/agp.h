@@ -332,6 +332,49 @@ int32_t agp_post_rand_grad(agp_post* p, int32_t layout, const void* Xs, int64_t 
                            const agp_noise* noise_s, const void* Z, int32_t S, const void* out_bar, double* grad_out,
                            void* noise_diag_out, void* mean_diag_out, void* y_bar_out, void* x_grad_out,
                            void* noise_s_diag_out, void* mean_s_diag_out, void* z_bar_out, void* xs_grad_out);
+/* Pullback of agp_post_mean_var at the cotangents mean_bar and var_bar of its two outputs: what reverse-mode AD returns
+ * through the reference's mean_and_var(posterior(fx, y)(x*, Sigma*)), for analytic acquisition functions (expected
+ * improvement, probability of improvement, UCB: closed forms in mu* and sigma^2 maximised over x*) and losses on
+ * predicted means.  p must come straight from agp_fit.  With C = K_xx + Sigma_y = L L', alpha = C^-1 (y - m),
+ * A = L^-1 K_xs and P = C^-1 K_xs = L^-T A, mu*_j = m*_j + (K_sx alpha)_j and sigma^2_j = k(x*_j, x*_j) - |A e_j|^2
+ * (+ sigma*^2_j); with mbar = mean_bar and vbar = var_bar these are agp_post_pred_logpdf_grad's formulas at
+ * mubar = mbar and Sigmabar = diag(vbar):
+ *   Kbar_sx[j, n] = mbar_j alpha_n - 2 vbar_j P[n, j],  beta = P mbar,  Cbar = P diag(vbar) P' - 1/2 (beta alpha' + alpha beta'),
+ *   ybar = beta,  mbar = -beta at x,  d/d sigma_i^2 = Cbar_ii,  d/d ConstMean c = sum mbar - sum beta,
+ *   xs_grad[j] = sum_n Kbar_sx[j, n] d1k(x*_j, x_n) + 2 vbar_j d1k(x*_j, x*_j)
+ * (d1 as agp_post_logpdf_grad_x's, through the Scale / ARD chain; the last term is nonzero only through Linear factors and
+ * products that contain them).  At x* the gradients with respect to the test mean and test noise are mbar and vbar
+ * themselves, so the call does not return them; neither the test mean nor the test noise enters the gradient, so the call
+ * takes neither.  A test point on a training point adds exactly 0 through every stationary factor (Matern 1/2: its zero
+ * subgradient, as agp_post_logpdf_grad_x).
+ * Inputs: Xs (M points in `layout`, as agp_post_mean_var's), mean_bar and var_bar (M values of the handle's dtype each;
+ * NULL means zeros).
+ * Outputs, each may be NULL and its work is then skipped: grad_out (double, the layout of agp_post_logpdf_grad: 5 + D for
+ * a single kernel, agp_post_grad_len(p) for a composite; [3] d/d sigma^2 of the training scalar noise, [4] d/d ConstMean
+ * c), noise_diag_out, mean_diag_out and y_bar_out (N values each), x_grad_out (N x D in `layout`) and xs_grad_out (M x D
+ * in `layout`).  Every output but grad_out has the handle's dtype; under AGP_MEM_DEVICE, Xs, mean_bar, var_bar and those
+ * outputs are DEVICE pointers.
+ * Routes, one per output: xs_grad_out always comes from one pass over the N x M pairs (x*_j, x_n) that forms Kbar_sx from
+ * P on the fly; grad_out, noise_diag_out and x_grad_out come from agp_post_pred_logpdf_grad's stacked reductions over
+ * [x; x*] with Sigmabar = diag(vbar); y_bar_out and mean_diag_out alone need only beta, one GEMV.  Passing NULL for every
+ * training-side output gives the test-side-only call an optimiser over x* needs.
+ * Cost: N^2 M for A (K_xs, then a multi-column forward substitution) and N^2 M for P (a backward substitution on L; both on
+ * the int8-sliced tensor cores above the substitutions' threshold), then N M D for the x* pass; when a kernel, noise or
+ * x output is asked for, 2 N M^2 for Kbar_sx, N^2 M for Cbar (the lower half) and the reductions over (N + M)^2 / 2 pairs.
+ * There is no N^3 or M^3 term: neither L^-1, C^-1 nor the posterior covariance is formed.
+ * Memory, besides the handle, in elements of the handle's dtype: about NM for A and P (P overwrites A) and O((N + M) D)
+ * for the x* pass when no kernel, noise or x output is asked for (no N x N or (N + M)^2 buffer); otherwise 2 NM briefly,
+ * then NM + M^2 + (N + M)^2 for P, Sigmabar and the stacked W.
+ * Arithmetic: the handle's dtype for K_xs, A, P and the products, fp64 for the x* pass (its weights and sums) and the
+ * reductions.  The fp32 error grows with cond(C) through P (DESIGN s6).
+ * Determinism: every per-point output and grad_out[3], grad_out[4] are formed in a fixed order (the x* pass writes
+ * per-CTA fp64 partials summed in a fixed order: two calls give the same bits); the other entries of grad_out leave their
+ * CTAs through fp64 atomics and agree to rounding.
+ * Errors: a bad layout or a NULL Xs: AGP_ERR_INVALID; M < 1: AGP_ERR_DIM_MISMATCH; an extended handle:
+ * AGP_ERR_UNSUPPORTED; a failed device allocation: AGP_ERR_CUDA.  VFE posteriors are not covered. */
+int32_t agp_post_mean_var_grad(agp_post* p, int32_t layout, const void* Xs, int64_t M, const void* mean_bar,
+                               const void* var_bar, double* grad_out, void* noise_diag_out, void* mean_diag_out,
+                               void* y_bar_out, void* x_grad_out, void* xs_grad_out);
 /* number of doubles agp_post_logpdf_grad writes: 5 + D for a single kernel, the layout above for a composite */
 int64_t agp_post_grad_len(const agp_post* p);
 /* V = U' \ B (N x nrhs, column-major): backs Xt_invA_X / diag_Xt_invA_X / Xt_invA_Y /

@@ -264,9 +264,12 @@ posterior(fx::DevFiniteGP{T}, y::AbstractVector{<:Real}) where {T} =
 
 # replaces src/exact_gpr_posterior.jl:85-90 (+ src/finite_gp_projection.jl:154-158) with the fused cross-Gram path
 const DevPosterior = PosteriorGP{<:GP,<:NamedTuple{(:α, :C, :x, :δ),<:Tuple{Any,DeviceCholesky,Any,Any}}}
-function mean_and_var(fx::FiniteGP{<:DevPosterior,<:DevInputs{T},<:Diagonal}) where {T}
+mean_and_var(fx::FiniteGP{<:DevPosterior,<:DevInputs{T},<:Diagonal}) where {T} = post_mean_var_primal(fx, false)
+# zero_mean: the means of the zero-mean prior at x* (the CustomMean split of the mean_and_var rule below)
+function post_mean_var_primal(fx::FiniteGP{<:DevPosterior,<:DevInputs{T},<:Diagonal}, zero_mean::Bool) where {T}
     p = fx.f; c = ctx(); Xs, layout, D = points(fx.x); M = length(fx)
-    ms, k2 = mean_spec(p.prior.mean, fx.x, T); ns, k3 = noise_spec(fx.Σy, T)
+    ms, k2 = zero_mean ? mean_spec(AbstractGPs.ZeroMean(), fx.x, T) : mean_spec(p.prior.mean, fx.x, T)
+    ns, k3 = noise_spec(fx.Σy, T)
     μ = Vector{T}(undef, M); v = Vector{T}(undef, M)
     lock(c.lock) do
         GC.@preserve Xs k2 k3 check(c, ccall((:agp_post_mean_var, libagp), Int32,
@@ -787,6 +790,66 @@ function CRC.rrule(config::CRC.RuleConfig{>:CRC.HasReverseMode}, ::typeof(Random
 end
 CRC.rrule(::typeof(zero_mean_post_rand), rng::Random.AbstractRNG, fx::DevPostFiniteGP, S::Int) =
     post_rand_rrule(rng, fx, S, true)
+
+# ---- reverse-mode rule for mean_and_var over a device posterior (analytic acquisition functions: expected improvement,
+# probability of improvement and UCB are closed forms in μ(x*) and σ²(x*), maximised over x*; marginals goes through it)
+# The forward pass is the primal method's (post_mean_var_primal, agp_post_mean_var); the pullback makes ONE
+# agp_post_mean_var_grad call with every output at the cotangents (m̄, v̄).  The tangents are those of the rand-over-posterior
+# rule: the kernel, data.x, data.δ = ȳ and data.C in the DevPosterior's tangent (the posterior rule routes them on); fx.x
+# gets the x* gradient and fx.Σy Diagonal(v̄), since the test noise adds to the variances.  A CustomMean prior goes through
+# AD of `mean_split_post_mean_var`: the closure's values at x* plus the device means and variances under a zero test mean
+# (`zero_mean_post_mean_var`, whose rule is the same pullback).
+zero_mean_post_mean_var(fx::DevPostFiniteGP) = post_mean_var_primal(fx, true)
+function mean_split_post_mean_var(fx::DevPostFiniteGP{T}) where {T}
+    μ0, v = zero_mean_post_mean_var(fx)
+    return T.(AbstractGPs.mean_vector(fx.f.prior.mean, fx.x)) .+ μ0, v
+end
+
+function post_mean_var_rrule(fx::DevPostFiniteGP{T}, zero_mean::Bool) where {T}
+    p = fx.f
+    μ, v = post_mean_var_primal(fx, zero_mean)
+    c = ctx(); Xs, layout, D = points(fx.x); M = length(fx)
+    X, xlayout, _ = points(p.data.x); N = p.data.C.n
+    composite = !supported(p.prior)
+    function post_mean_var_pullback(Δ)
+        Δ = CRC.unthunk(Δ)
+        Δ isa CRC.AbstractZero && return CRC.NoTangent(), CRC.ZeroTangent()
+        m̄ = notangent(Δ[1]) ? zeros(T, M) : convert(Vector{T}, CRC.unthunk(Δ[1]))
+        v̄ = notangent(Δ[2]) ? zeros(T, M) : convert(Vector{T}, CRC.unthunk(Δ[2]))
+        glen = composite ? ccall((:agp_post_grad_len, libagp), Int64, (Ptr{Cvoid},), p.data.C.h) : 5 + D
+        g = Vector{Float64}(undef, glen); nd = Vector{T}(undef, N); ȳ = Vector{T}(undef, N)
+        xg = X isa AbstractVector || xlayout == layout ? similar(X, T) : similar(permutedims(X), T)
+        xsg = similar(Xs, T)
+        lock(c.lock) do
+            GC.@preserve Xs m̄ v̄ g nd ȳ xg xsg check(c, ccall((:agp_post_mean_var_grad, libagp), Int32,
+                (Ptr{Cvoid}, Int32, Ptr{Cvoid}, Int64, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Float64}, Ptr{Cvoid}, Ptr{Cvoid}, Ptr{Cvoid},
+                 Ptr{Cvoid}, Ptr{Cvoid}),
+                p.data.C.h, layout, Xs, M, m̄, v̄, g, nd, C_NULL, ȳ, xg, xsg))
+        end
+        # grad_out[5] is d/dc through both sides; the prior mean's tangent keeps the test side, data.δ carries the rest
+        gs = (variance=g[1], scale=g[2], linear_c=g[3], noise=g[4], mean_c=g[5] + sum(ȳ), ard=g[6:end], noise_diag=nd)
+        if composite
+            kt = ctangent(p.prior.kernel, Int[], composite_grads(p.prior.kernel, D, g), 1.0)
+        else
+            _, var, _, wt = flat(p.prior.kernel)
+            kt = kernel_tangent(p.prior.kernel, gs, var, wt === nothing ? 1.0 : wt)
+        end
+        mt = zero_mean ? CRC.NoTangent() : mean_tangent(p.prior.mean, gs)
+        p̄rior = CRC.Tangent{typeof(p.prior)}(; mean=mt, kernel=kt)
+        d̄ata = CRC.Tangent{typeof(p.data)}(; C=(noise=g[4], noise_diag=nd),
+                                            x=x_tangent(p.data.x, as_storage(xg, X, layout, xlayout)), δ=ȳ)
+        f̄ = CRC.Tangent{typeof(p)}(; prior=p̄rior, data=d̄ata)
+        f̄x = CRC.Tangent{typeof(fx)}(; f=f̄, x=x_tangent(fx.x, xsg), Σy=noise_tangent(fx.Σy, (noise=sum(v̄), noise_diag=v̄)))
+        return CRC.NoTangent(), f̄x
+    end
+    return (μ, v), post_mean_var_pullback
+end
+
+function CRC.rrule(config::CRC.RuleConfig{>:CRC.HasReverseMode}, ::typeof(mean_and_var), fx::DevPostFiniteGP{T}) where {T}
+    fx.f.prior.mean isa AbstractGPs.CustomMean && return CRC.rrule_via_ad(config, mean_split_post_mean_var, fx)
+    return post_mean_var_rrule(fx, false)
+end
+CRC.rrule(::typeof(zero_mean_post_mean_var), fx::DevPostFiniteGP) = post_mean_var_rrule(fx, true)
 
 # ---- reverse-mode rules for the VFE objectives: elbo(VFE(fz), fx, y) and approx_log_evidence(VFE | DTC, fx, y) ---------
 # (src/sparse_approximations.jl:248-254, :282-286).  One agp_vfe_elbo_grad_x call returns the value, the kernel / noise /
