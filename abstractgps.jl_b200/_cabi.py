@@ -20,6 +20,7 @@ AGP_MEM_HOST, AGP_MEM_DEVICE = 0, 1
 
 AGP_RQ, AGP_PERIODIC, AGP_WHITE, AGP_CONSTANT, AGP_COMPOSITE = 5, 6, 7, 8, 9
 AGP_COMPOSITE_MAX = 8  # terms, and factors in all
+AGP_PANEL_SPLIT_SUBST, AGP_PANEL_SPLIT_GEMM, AGP_PANEL_FUSED = 0, 1, 2
 
 
 class agp_kernel_factor(C.Structure):
@@ -117,6 +118,10 @@ SIGNATURES = {
                                              C.c_int32, C.c_int64, C.c_int64, C.c_int64, C.c_int64]),
     "agp_debug_ozaki8": (C.c_int32, [_P, _P, C.c_int64, _P, C.c_int32, C.c_int64, C.c_int64, _P, C.c_int32, C.c_int64,
                                      C.c_int64, C.c_int64, C.c_int32, C.c_double, C.c_int64, C.c_int64, C.c_int64, C.c_int64]),
+    "agp_debug_gemm": (C.c_int32, [_P, C.c_int32, _P, C.c_int32, C.c_int64, _P, C.c_int32, C.c_int64, _P, C.c_int64,
+                                   C.c_int64, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int64,
+                                   C.c_int64, C.c_int64]),
+    "agp_debug_panel": (C.c_int32, [_P, C.c_int32, C.c_int32, _P, C.c_int64, C.c_int64, C.c_int32, _P, _P, _P]),
     "agp_bc_owner": (C.c_int32, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
     "agp_bc_local_tiles": (C.c_int64, [C.c_int32, C.c_int32, C.c_int32, C.c_int32]),
 }

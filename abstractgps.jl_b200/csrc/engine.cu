@@ -353,7 +353,7 @@ void trailing_update(agp_ctx* ctx, T* L, int64_t lda, int64_t row0, int64_t col0
   if (!done) {
     GemmArgs u{};
     u.A = L + row0 + kcol0 * lda; u.lda = lda;
-    u.B = L + col0 + kcol0 * lda; u.ldb = lda;
+    u.B = L + row0 + kcol0 * lda; u.ldb = lda;  // column n reads panel row row0 + n, or col0 + n through the map
     u.C = L + row0 + col0 * lda; u.ldc = lda;
     u.M = M; u.N = N; u.K = K; u.alpha_neg = 1; u.beta_one = 1; u.lower_only = 1;
     if (row0 != col0) { u.b_tile_stride = TILE; u.b_off = col0 - row0; }  // lower-only test relative to row0
@@ -421,57 +421,65 @@ template <typename T> static bool ensure_oz(agp_ctx* ctx, int64_t rows, int K, b
   return ensure_ws(ctx->oz, ctx->oz_rows, rows, K, slice_format<T>(ctx, K, factor), s);
 }
 
+// the route of one panel step: the fp64 split kernels (AGP_POTRF_SPLIT, default on) solve a panel of fewer than
+// AGP_TRSM_GEMM_MIN rows below the block by substitution, a taller one by the strip inverse and one in-place GEMM
+template <typename T>
+int panel_route(int64_t rows_below) {
+  if (!std::is_same<T, double>::value || !potrf_split_enabled()) return AGP_PANEL_FUSED;
+  static const int64_t trsm_gemm_min = env_int64("AGP_TRSM_GEMM_MIN", 8192);
+  return rows_below >= trsm_gemm_min ? AGP_PANEL_SPLIT_GEMM : AGP_PANEL_SPLIT_SUBST;
+}
+
+// factor the 128 x 128 block at Akk in place and solve the rows_below panel rows under it, A21 <- A21 L11^-T, by `route`;
+// Dinv_k receives inv(L11).  The substitution route leaves the inverse on stream3 (joined by join_inverses).
+template <typename T>
+void panel_block(agp_ctx* ctx, int route, T* Akk, int64_t lda, int64_t rows_below, T* Dinv_k, double* logdet_part,
+                 int blk, int* info, cudaStream_t s) {
+  if constexpr (std::is_same<T, double>::value) {
+    if (route == AGP_PANEL_SPLIT_SUBST) {
+      // short panels (latency-bound): factor on the main stream; the inverse (only the solves need it) on stream3;
+      // the panel TRSM by blocked substitution straight from L11
+      launch_potrf_factor_f64(Akk, lda, logdet_part, blk, info, s);
+      cudaEventRecord(ctx->ev_fac, s);
+      cudaStreamWaitEvent(ctx->stream3, ctx->ev_fac, 0);
+      launch_trtri_f64(Akk, lda, Dinv_k, ctx->stream3);
+      ctx->s3_dirty = true;
+      if (rows_below > 0) launch_trsm_sub_f64(Akk + TILE, lda, rows_below, Akk, s);
+      return;
+    }
+    if (route == AGP_PANEL_SPLIT_GEMM) {
+      // tall panels: the substitution kernel (32 rows per CTA, 16 dependent steps) runs at ~4 TFLOP/s; the 128x128
+      // inverse (8 CTAs, 14 us) followed by ONE in-place DMMA GEMM A21 <- A21 inv(L11)' is ~3x faster from ~8k rows
+      launch_potrf_factor_f64(Akk, lda, logdet_part, blk, info, s);
+      launch_trtri_f64(Akk, lda, Dinv_k, s);
+    }
+  }
+  if (route == AGP_PANEL_FUSED) launch_potrf_diag<T>(Akk, lda, Dinv_k, logdet_part, blk, info, s);
+  if (rows_below > 0) {
+    GemmArgs t{};  // A21 <- A21 * inv(L11)'
+    t.A = Akk + TILE; t.lda = lda; t.B = Dinv_k; t.ldb = TILE;
+    t.C = Akk + TILE; t.ldc = lda; t.M = rows_below; t.N = TILE; t.K = TILE;
+    launch_gemm<T>(t, s);
+  }
+}
+
 // factor one outer panel in place: Lp points at its diagonal element; Gp inner 128-blocks; rows = rows from the
 // panel's first row to the end of the (local) column storage (border rows included)
 template <typename T>
 void factor_panel_step(agp_ctx* ctx, T* Lp, int64_t lda, int Gp, int g, int64_t rows, T* Dinv_p, double* logdet_part,
                        int blk_base, int* info, cudaStream_t s) {
-  {
-    T* Akk = Lp + (int64_t)g * TILE + (int64_t)g * TILE * lda;
-    const int64_t rows_below = rows - (int64_t)(g + 1) * TILE;
-    bool split_done = false;
-    if constexpr (std::is_same<T, double>::value) {
-      if (potrf_split_enabled()) {
-        launch_potrf_factor_f64(Akk, lda, logdet_part, blk_base + g, info, s);
-        static const int64_t trsm_gemm_min = env_int64("AGP_TRSM_GEMM_MIN", 8192);
-        if (rows_below >= trsm_gemm_min) {
-          // tall panels: the substitution kernel (32 rows per CTA, 16 dependent steps) runs at ~4 TFLOP/s; the 128x128
-          // inverse (8 CTAs, 14 us) followed by ONE in-place DMMA GEMM A21 <- A21 inv(L11)' is ~3x faster from ~8k rows
-          launch_trtri_f64(Akk, lda, Dinv_p + (int64_t)g * TILE * TILE, s);
-          GemmArgs t{};
-          t.A = Akk + TILE; t.lda = lda; t.B = Dinv_p + (int64_t)g * TILE * TILE; t.ldb = TILE;
-          t.C = Akk + TILE; t.ldc = lda; t.M = rows_below; t.N = TILE; t.K = TILE;
-          launch_gemm<T>(t, s);
-        } else {
-          // short panels (latency-bound): factor on the main stream; the inverse (only the solves need it) on stream3;
-          // the panel TRSM by blocked substitution straight from L11
-          cudaEventRecord(ctx->ev_fac, s);
-          cudaStreamWaitEvent(ctx->stream3, ctx->ev_fac, 0);
-          launch_trtri_f64(Akk, lda, Dinv_p + (int64_t)g * TILE * TILE, ctx->stream3);
-          ctx->s3_dirty = true;
-          if (rows_below > 0) launch_trsm_sub_f64(Akk + TILE, lda, rows_below, Akk, s);
-        }
-        split_done = true;
-      }
-    }
-    if (!split_done) {
-      launch_potrf_diag<T>(Akk, lda, Dinv_p + (int64_t)g * TILE * TILE, logdet_part, blk_base + g, info, s);
-      if (rows_below > 0) {
-        GemmArgs t{};  // A21 <- A21 * inv(L11)'
-        t.A = Akk + TILE; t.lda = lda; t.B = Dinv_p + (int64_t)g * TILE * TILE; t.ldb = TILE;
-        t.C = Akk + TILE; t.ldc = lda; t.M = rows_below; t.N = TILE; t.K = TILE;
-        launch_gemm<T>(t, s);
-      }
-    }
-    if (rows_below <= 0) return;
-    const int64_t ncols_in = (int64_t)(Gp - (g + 1)) * TILE;  // rank-128 update of the remaining inner columns
-    if (ncols_in > 0) {
-      GemmArgs u{};
-      u.A = Akk + TILE; u.lda = lda; u.B = Akk + TILE; u.ldb = lda;
-      u.C = Akk + TILE + (int64_t)TILE * lda; u.ldc = lda;
-      u.M = rows_below; u.N = ncols_in; u.K = TILE; u.alpha_neg = 1; u.beta_one = 1; u.lower_only = 1;
-      launch_gemm<T>(u, s);
-    }
+  T* Akk = Lp + (int64_t)g * TILE + (int64_t)g * TILE * lda;
+  const int64_t rows_below = rows - (int64_t)(g + 1) * TILE;
+  panel_block<T>(ctx, panel_route<T>(rows_below), Akk, lda, rows_below, Dinv_p + (int64_t)g * TILE * TILE, logdet_part,
+                 blk_base + g, info, s);
+  if (rows_below <= 0) return;
+  const int64_t ncols_in = (int64_t)(Gp - (g + 1)) * TILE;  // rank-128 update of the remaining inner columns
+  if (ncols_in > 0) {
+    GemmArgs u{};
+    u.A = Akk + TILE; u.lda = lda; u.B = Akk + TILE; u.ldb = lda;
+    u.C = Akk + TILE + (int64_t)TILE * lda; u.ldc = lda;
+    u.M = rows_below; u.N = ncols_in; u.K = TILE; u.alpha_neg = 1; u.beta_one = 1; u.lower_only = 1;
+    launch_gemm<T>(u, s);
   }
 }
 
@@ -3961,6 +3969,58 @@ int32_t agp_debug_ozaki8(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* A_d
   if (e == cudaSuccess) e = cudaGetLastError();
   if (e != cudaSuccess) { ctx->err = std::string("ozaki8: ") + cudaGetErrorString(e); return AGP_ERR_CUDA; }
   if (urc) { ctx->err = "ozaki8: K above 16384 or strip table not supported"; return AGP_ERR_UNSUPPORTED; }
+  return AGP_OK;
+}
+
+int32_t agp_debug_gemm(agp_ctx* ctx, int32_t dtype, const void* A_dev, int32_t a_kmajor, int64_t lda, const void* B_dev,
+                       int32_t b_kmajor, int64_t ldb, void* C_dev, int64_t ldc, int64_t M, int64_t N, int64_t K,
+                       int32_t alpha_neg, int32_t beta_one, int32_t lower_only, int32_t trmm_lower, int64_t b_tile_stride,
+                       int64_t b_tile_width, int64_t b_off) {
+  if (!ctx || !A_dev || !B_dev || !C_dev) return AGP_ERR_INVALID;
+  if (dtype != AGP_F32 && dtype != AGP_F64) { ctx->err = "gemm: dtype must be AGP_F32 or AGP_F64"; return AGP_ERR_INVALID; }
+  cudaSetDevice(ctx->device);
+  GemmArgs g{};
+  g.A = A_dev; g.lda = lda; g.a_kmajor = a_kmajor != 0;
+  g.B = B_dev; g.ldb = ldb; g.b_kmajor = b_kmajor != 0;
+  g.C = C_dev; g.ldc = ldc; g.M = M; g.N = N; g.K = K;
+  g.alpha_neg = alpha_neg != 0; g.beta_one = beta_one != 0; g.lower_only = lower_only != 0; g.trmm_lower = trmm_lower != 0;
+  g.b_tile_stride = b_tile_stride; g.b_tile_width = b_tile_width; g.b_off = b_off;
+  const int rc = dtype == AGP_F64 ? launch_gemm<double>(g, ctx->stream) : launch_gemm<float>(g, ctx->stream);
+  if (rc) { ctx->err = "gemm: the operands break the tile GEMM's contract (csrc/kernels.h)"; return AGP_ERR_INVALID; }
+  cudaError_t e = cudaStreamSynchronize(ctx->stream);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) { ctx->err = std::string("gemm: ") + cudaGetErrorString(e); return AGP_ERR_CUDA; }
+  return AGP_OK;
+}
+
+int32_t agp_debug_panel(agp_ctx* ctx, int32_t dtype, int32_t route, void* A_dev, int64_t lda, int64_t rows_below,
+                        int32_t blk, void* Dinv_dev, double* logdet_dev, int32_t* info_dev) {
+  if (!ctx || !A_dev || !Dinv_dev || !logdet_dev || !info_dev) return AGP_ERR_INVALID;
+  if (dtype != AGP_F32 && dtype != AGP_F64) { ctx->err = "panel: dtype must be AGP_F32 or AGP_F64"; return AGP_ERR_INVALID; }
+  if (route != AGP_PANEL_FUSED && (dtype != AGP_F64 || (route != AGP_PANEL_SPLIT_SUBST && route != AGP_PANEL_SPLIT_GEMM))) {
+    ctx->err = "panel: the split routes are fp64 only";
+    return AGP_ERR_INVALID;
+  }
+  // the panel GEMM reads A21 and Dinv in 16-byte loads (the GemmArgs contract)
+  const int64_t vec = dtype == AGP_F64 ? 2 : 4;
+  if (rows_below < 0 || blk < 0 || lda < TILE + rows_below || lda % vec || ((uintptr_t)A_dev & 15) ||
+      ((uintptr_t)Dinv_dev & 15)) {
+    ctx->err = "panel: need 0 <= rows_below <= lda - 128, blk >= 0, lda and the pointers aligned to 16 bytes";
+    return AGP_ERR_INVALID;
+  }
+  if (dtype == AGP_F32 && rows_below % 4) {  // the fp32 panel GEMM stores float4 row quads (M % 4 == 0)
+    ctx->err = "panel: an fp32 panel needs rows_below % 4 == 0";
+    return AGP_ERR_INVALID;
+  }
+  cudaSetDevice(ctx->device);
+  if (dtype == AGP_F64)
+    panel_block<double>(ctx, route, (double*)A_dev, lda, rows_below, (double*)Dinv_dev, logdet_dev, blk, info_dev, ctx->stream);
+  else
+    panel_block<float>(ctx, route, (float*)A_dev, lda, rows_below, (float*)Dinv_dev, logdet_dev, blk, info_dev, ctx->stream);
+  join_inverses(ctx);
+  cudaError_t e = cudaStreamSynchronize(ctx->stream);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  if (e != cudaSuccess) { ctx->err = std::string("panel: ") + cudaGetErrorString(e); return AGP_ERR_CUDA; }
   return AGP_OK;
 }
 

@@ -305,20 +305,43 @@ static void launch_dmma(const GemmArgs& g, cudaStream_t s) {
   agp_count_launch();
 }
 
+// The operand contract of GemmArgs (kernels.h) for the instantiation a product selects; tbn is its column-tile width.
+template <typename T>
+static bool gemm_contract_ok(const GemmArgs& g, int64_t tbn) {
+  constexpr int64_t V = 16 / sizeof(T);  // elements per 16-byte load
+  auto aligned = [](const void* p) { return ((uintptr_t)p & 15) == 0; };
+  if (g.K < 0 || !aligned(g.A) || !aligned(g.B) || g.lda % V || g.ldb % V) return false;
+  if (sizeof(T) == 4 && (!aligned(g.C) || g.ldc % V || g.M % V)) return false;  // float4 epilogue
+  if ((g.a_kmajor || g.b_kmajor) && g.K % V) return false;  // a K-major load reads k .. k + V - 1 and checks only k
+  const int64_t bw = g.b_tile_width ? g.b_tile_width : 128;
+  int64_t n_hi = g.N - 1;  // highest B column read
+  if (g.b_tile_stride) {
+    if (g.b_tile_stride < 0 || g.b_tile_width < 0 || g.b_off < 0 || bw % tbn) return false;
+    if (!g.b_kmajor && ((g.b_tile_stride - bw) % V || g.b_off % V)) return false;  // the shift keeps B's loads aligned
+    const int64_t blk = n_hi / bw;
+    n_hi = blk * g.b_tile_stride + n_hi % bw;
+    if (blk > 0 && (blk - 1) * g.b_tile_stride + bw - 1 > n_hi) n_hi = (blk - 1) * g.b_tile_stride + bw - 1;
+    n_hi += g.b_off;
+  }
+  if (g.lda < (g.a_kmajor ? g.K : g.M) || g.ldb < (g.b_kmajor ? g.K : n_hi + 1) || g.ldc < g.M) return false;
+  // in place: one CTA owns every row (C == A) or column (C == B) it reads, and reads them all before it writes
+  if (g.C == g.A && (g.a_kmajor || g.ldc != g.lda || g.N > 128)) return false;
+  if (g.C == g.B && (!g.b_kmajor || g.ldc != g.ldb || g.M > 128 || g.b_tile_stride)) return false;
+  return true;
+}
+
 template <>
-void launch_gemm<double>(const GemmArgs& g, cudaStream_t s) {
-  if (g.M <= 0 || g.N <= 0) return;
+int launch_gemm<double>(const GemmArgs& g, cudaStream_t s) {
+  if (g.M <= 0 || g.N <= 0) return 0;
+  if (!gemm_contract_ok<double>(g, (g.C == g.A || g.C == g.B) ? 128 : 64)) return 1;
   // in-place products (C aliases an operand) need one CTA to own every column it reads: 128-wide tile.
   // C == A (panel TRSM): 64 x 128 tiles, 2 CTAs/SM -- twice the CTAs on the latency-critical panel solve.
+  // The contract leaves A MN-major when C == A and B K-major when C == B.
   if (g.C == g.A) {
-    if (!g.a_kmajor && !g.b_kmajor) launch_dmma<false, false, 1, 4>(g, s);
-    else if (!g.a_kmajor && g.b_kmajor) launch_dmma<false, true, 1, 4>(g, s);
-    else if (g.a_kmajor && !g.b_kmajor) launch_dmma<true, false, 1, 4>(g, s);
-    else launch_dmma<true, true, 1, 4>(g, s);
+    if (!g.b_kmajor) launch_dmma<false, false, 1, 4>(g, s);
+    else launch_dmma<false, true, 1, 4>(g, s);
   } else if (g.C == g.B) {
-    if (!g.a_kmajor && !g.b_kmajor) launch_dmma<false, false, 2, 4>(g, s);
-    else if (!g.a_kmajor && g.b_kmajor) launch_dmma<false, true, 2, 4>(g, s);
-    else if (g.a_kmajor && !g.b_kmajor) launch_dmma<true, false, 2, 4>(g, s);
+    if (!g.a_kmajor) launch_dmma<false, true, 2, 4>(g, s);
     else launch_dmma<true, true, 2, 4>(g, s);
   } else {  // (64x64 tiles for the narrow next-column update were measured: 21 us vs 19 us for 128x64 -- not kept)
     if (!g.a_kmajor && !g.b_kmajor) launch_dmma<false, false, 2, 2>(g, s);
@@ -326,13 +349,16 @@ void launch_gemm<double>(const GemmArgs& g, cudaStream_t s) {
     else if (g.a_kmajor && !g.b_kmajor) launch_dmma<true, false, 2, 2>(g, s);
     else launch_dmma<true, true, 2, 2>(g, s);
   }
+  return 0;
 }
 
 template <>
-void launch_gemm<float>(const GemmArgs& g, cudaStream_t s) {
-  if (g.M <= 0 || g.N <= 0) return;
+int launch_gemm<float>(const GemmArgs& g, cudaStream_t s) {
+  if (g.M <= 0 || g.N <= 0) return 0;
+  if (!gemm_contract_ok<float>(g, BN)) return 1;
   if (!g.a_kmajor && !g.b_kmajor) launch_cfg(gemm_simt_kernel<false, false>, g, 0, s);
   else if (!g.a_kmajor && g.b_kmajor) launch_cfg(gemm_simt_kernel<false, true>, g, 0, s);
   else if (g.a_kmajor && !g.b_kmajor) launch_cfg(gemm_simt_kernel<true, false>, g, 0, s);
   else launch_cfg(gemm_simt_kernel<true, true>, g, 0, s);
+  return 0;
 }

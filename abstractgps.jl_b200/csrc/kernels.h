@@ -54,6 +54,19 @@ struct GramParams {
 };
 
 // op(A) is M x K, op(B) is K x N, C is M x N (ldc).  C = beta*C + alpha*op(A)op(B), alpha in {+1,-1}.
+// Contract (launch_gemm checks it on the host and launches nothing, returning nonzero, when it fails):
+//  - A and B 16-byte aligned, lda and ldb even (fp64) or multiples of 4 (fp32): the operands are read in 16-byte loads;
+//    fp32 also needs C 16-byte aligned, ldc % 4 == 0 and M % 4 == 0 (the epilogue stores float4 and checks only m < M);
+//  - lda >= K (A K-major) or M, ldb >= K (B K-major) or 1 + the highest B column the column map reads, ldc >= M;
+//  - K even (fp64) or K % 4 == 0 (fp32) when either operand is K-major: a load of k .. k+1 (k+3) checks only k < K, and
+//    a NaN past K times the other operand's zero fill would still poison the sum;
+//  - C == A: a_kmajor = 0, ldc == lda, N <= 128; C == B: b_kmajor = 1, ldc == ldb, M <= 128, no column map.  One CTA then
+//    owns every row (column) of the aliased operand it reads and reads all of them before its epilogue;
+//  - column map: stride, width and b_off >= 0, the width a multiple of the instantiation's column tile (fp64: 128 when C
+//    aliases an operand, else 64; fp32: 128), and for an MN-major B the shift a multiple of the load width.
+// C overlapping an operand only partly (sharing columns but not rows, say) is the caller's business and is not checked.
+// Tiles: fp64 64 x 128 (C == A), 128 x 128 (C == B), 128 x 64 otherwise; fp32 128 x 128.  lower_only skips whole tiles,
+// trmm_lower cuts K at the end of the row tile, so A is read above its diagonal inside the tile's band.
 struct GemmArgs {
   const void* A; int64_t lda; int a_kmajor;  // 0: A(m,k) at A[m + k*lda]   1: A(m,k) at A[k + m*lda]
   const void* B; int64_t ldb; int b_kmajor;  // 0: B(k,n) at B[n + k*ldb]   1: B(k,n) at B[k + n*ldb]
@@ -88,9 +101,11 @@ template <typename T> void launch_border_init_cols(T* A, int64_t lda, int64_t ro
                                                    double mean_c, const T* mean_v, cudaStream_t s);
 // diagonal block factorisation + inverse: A (TILE x TILE at Ablk, lda) -> L in place (upper zeroed),
 // Dinv = inv(L) (TILE x TILE col-major, lower), logdet_part[blk] = sum log L_jj, info (first bad pivot, 1-based).
+// One fused kernel; the fp64 factorisation uses it only on the AGP_PANEL_FUSED route (agp.h), the split kernels below
+// otherwise.
 template <typename T> void launch_potrf_diag(T* Ablk, int64_t lda, T* Dinv, double* logdet_part, int blk,
                                              int* info, cudaStream_t s);
-template <typename T> void launch_gemm(const GemmArgs& g, cudaStream_t s);
+template <typename T> int launch_gemm(const GemmArgs& g, cudaStream_t s);  // 0: launched (or nothing to do); else refused
 // fp64 split schedule: factor-only diagonal block, 8-CTA strip inverse (off the critical path), and the
 // panel TRSM by blocked substitution that does not need the 128x128 inverse
 int potrf_split_enabled();

@@ -20,18 +20,22 @@ constexpr int PLD = PB + 1;   // odd leading dimension -> conflict-free column/r
 
 // 1/sqrt(p) on the critical path of the column chain: hardware approximation (MUFU.RSQ64H, ~20 bits)
 // + two Newton steps (3 dependent DFMA-class ops each) -> full fp64 precision, ~half the dependent
-// depth of rsqrt(double)'s library sequence.  p is a positive, normal pivot.
+// depth of rsqrt(double)'s library sequence.  p is a positive pivot.  The approximation flushes a subnormal input to
+// zero (+Inf, then NaN after the Newton steps), so a subnormal p is scaled by 2^108 first and the result by 2^54; both
+// scalings are exact, and a normal p takes the unscaled path unchanged.
 template <typename T> __device__ __forceinline__ T dev_rsqrt_refined(T p);
 template <> __device__ __forceinline__ double dev_rsqrt_refined<double>(double p) {
+  const bool sub = p < 0x1p-1022;
+  const double ps = sub ? p * 0x1p+108 : p;
   double y;
-  asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(p));
-  const double hp = -0.5 * p;
+  asm("rsqrt.approx.ftz.f64 %0, %1;" : "=d"(y) : "d"(ps));
+  const double hp = -0.5 * ps;
 #pragma unroll
   for (int it = 0; it < 2; ++it) {
     const double e = fma(hp * y, y, 0.5);  // 0.5 - 0.5 p y^2
     y = fma(y, e, y);                      // y (1.5 - 0.5 p y^2)
   }
-  return y;
+  return sub ? y * 0x1p+54 : y;
 }
 template <> __device__ __forceinline__ float dev_rsqrt_refined<float>(float p) {
   float r = rsqrtf(p);
@@ -815,21 +819,10 @@ void launch_potrf_diag<double>(double* Ablk, int64_t lda, double* Dinv, double* 
                                cudaStream_t s) {
   const size_t smem = (size_t)(PB * PLD + PB * XLD + 64 + 8 + PB) * sizeof(double);
   static uint64_t configured = 0;  // per-device bit: the attribute is per device (one ctx per GPU in one process)
-  static int split = 1;
   if (agp_first_use_on_device(&configured)) {
     cudaFuncSetAttribute(potrf_diag_kernel_f64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(potrf_factor_only_f64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    cudaFuncSetAttribute(trtri_strips_f64, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    const char* v = getenv("AGP_POTRF_SPLIT");
-    if (v) split = atoi(v);
   }
-  if (split) {  // factor on one CTA (critical path), inverse on 8 CTAs
-    potrf_factor_only_f64<<<1, 256, smem, s>>>(Ablk, lda, logdet_part, blk, info);
-    trtri_strips_f64<<<8, 256, smem, s>>>(Ablk, lda, Dinv);
-    agp_count_launch();
-  } else {
-    potrf_diag_kernel_f64<<<1, 256, smem, s>>>(Ablk, lda, Dinv, logdet_part, blk, info);
-  }
+  potrf_diag_kernel_f64<<<1, 256, smem, s>>>(Ablk, lda, Dinv, logdet_part, blk, info);
   agp_count_launch();
 }
 

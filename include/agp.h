@@ -540,6 +540,30 @@ int32_t agp_debug_ozaki8(agp_ctx* ctx, void* C_dev, int64_t ldc, const void* A_d
                          int64_t m_panel, const void* B_dev, int32_t b_kmajor, int64_t ldb, int64_t M, int64_t N, int32_t K,
                          double sign, int64_t b_tile_stride, int64_t b_tile_width, int64_t b_off, int64_t a_off);
 
+/* ---- test hook for the tile GEMM (csrc/gemm.cu): DEVICE pointers, dtype AGP_F32 | AGP_F64, one launch on the caller's
+ * buffers.  C (M x N, ldc) = beta C + alpha op(A) op(B), alpha = -1 if alpha_neg else +1, beta = 1 if beta_one else 0;
+ * A(m,k) at A[m + k*lda] (a_kmajor = 0) or A[k + m*lda]; B(k,n) at B[n + k*ldb] (b_kmajor = 0) or B[k + n*ldb].  C == A
+ * or C == B (the same pointer) selects the in-place kernels.  lower_only skips tiles above the diagonal, trmm_lower
+ * reads A as lower triangular (K cut at the end of each row tile); column n of C takes B's column
+ * (n / w) * b_tile_stride + n % w + b_off (w = b_tile_width, 0 -> 128) when b_tile_stride != 0.  Operands that break
+ * the contract of GemmArgs (csrc/kernels.h) are refused with AGP_ERR_INVALID before anything is launched. */
+int32_t agp_debug_gemm(agp_ctx* ctx, int32_t dtype, const void* A_dev, int32_t a_kmajor, int64_t lda, const void* B_dev,
+                       int32_t b_kmajor, int64_t ldb, void* C_dev, int64_t ldc, int64_t M, int64_t N, int64_t K,
+                       int32_t alpha_neg, int32_t beta_one, int32_t lower_only, int32_t trmm_lower, int64_t b_tile_stride,
+                       int64_t b_tile_width, int64_t b_off);
+
+/* routes of one step of the blocked Cholesky: how the 128 x 128 diagonal block is factored and the panel below it solved */
+#define AGP_PANEL_SPLIT_SUBST 0 /* fp64: factor-only kernel, panel by blocked substitution, inverse on a side stream */
+#define AGP_PANEL_SPLIT_GEMM 1  /* fp64: factor-only kernel, strip inverse, panel by one in-place GEMM with the inverse */
+#define AGP_PANEL_FUSED 2       /* fused factor + inverse kernel, panel by the in-place GEMM (fp32's only route) */
+/* ---- test hook for one panel step (csrc/potrf.cu): DEVICE pointers.  Factors the 128 x 128 block at A (lda, lower
+ * triangle read) in place (L, upper triangle zeroed), solves the rows_below rows under it, A21 <- A21 L^-T, and writes
+ * Dinv (128 x 128, = inv(L)), logdet[blk] = sum_j log L_jj and, at the first non-positive pivot j (1-based) of the
+ * block, info = blk * 128 + j unless info is already nonzero.  Returns once every stream has finished.  fp32 panels need
+ * rows_below % 4 == 0 (the panel GEMM's contract; AGP_ERR_INVALID otherwise, before anything runs). */
+int32_t agp_debug_panel(agp_ctx* ctx, int32_t dtype, int32_t route, void* A_dev, int64_t lda, int64_t rows_below,
+                        int32_t blk, void* Dinv_dev, double* logdet_dev, int32_t* info_dev);
+
 /* ---- host-only helpers of the 2D block-cyclic tile map (no GPU needed; used by the CPU
  * world_size-2 tests): owner rank of tile (i,j) on a P x Q grid and local tile counts. */
 int32_t agp_bc_owner(int32_t ti, int32_t tj, int32_t grid_p, int32_t grid_q);
