@@ -22,8 +22,12 @@
 // stack of B slices would write overlapping accumulator fragments of different widths, which ptxas serialises.  The
 // fragments are double-buffered so one chunk's MMAs stay in flight while the next chunk's fragments load.  The S
 // accumulator blocks of 64 x BN int32 live in registers (S*BN/2 per thread), which sets BN: 64 for S <= 4, 32 above.
-// The producer also stages the tile's old C block into shared memory halfway through the tile's K loop, so the drain's
-// read-modify-write does not wait on HBM (partial or unaligned tiles read C from global memory as before).
+// The eight-bit kernel instead reads A from shared memory too (oz_chunk_ss): without fragments its six blocks of 64 x 64
+// fit, and the wider tile fetches each 128-row A chunk once per 64 columns instead of once per 32 (-40 % operand bytes).
+// A from registers would need two fragment buffers (48 registers) beside the 192 accumulators to keep a chunk's MMAs in
+// flight while the next chunk's fragments load, more than a consumer thread has.  The producer also stages the tile's
+// old C block into shared memory halfway through the tile's K loop, so the drain's read-modify-write does not wait on
+// HBM (partial or unaligned tiles read C from global memory as before).
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <math_constants.h>
@@ -242,11 +246,12 @@ struct OzTileArgs {
   int c_bulk;                    // C and ldc 16-byte aligned: full tiles stage their C block by bulk copies
 };
 
-// per slice count and C type: output tile 128 x BN, pipeline depth, staged C block (column-major, every column padded
-// by 16 bytes so the drain's shared-memory reads are free of bank conflicts)
-template <int S, typename CT>
+// per slice count, digit width and C type: output tile 128 x BN, pipeline depth, staged C block (column-major, every
+// column padded by 16 bytes so the drain's shared-memory reads are free of bank conflicts).  Eight-bit digits take both
+// operands from shared memory, which frees the A fragment registers for 128 x 64 tiles (four stages of 36 KB).
+template <int S, int BITS, typename CT>
 struct OzCfg {
-  static constexpr int BN = (S <= 4) ? 64 : 32;
+  static constexpr int BN = (S <= 4 || BITS == 8) ? 64 : 32;
   static constexpr int A_BYTES = OZ_BM * OZ_KC, B_BYTES = BN * OZ_KC;
   static constexpr int STAGE_BYTES = S * (A_BYTES + B_BYTES);
   static constexpr int C_LD = OZ_BM + 16 / (int)sizeof(CT);  // elements per staged C column
@@ -379,6 +384,22 @@ __device__ __forceinline__ void oz_chunk(uint32_t* acc, uint32_t (&af)[S][4], ui
   wgmma_commit();
 }
 
+// the same chunk with both operands in shared memory (128 x 64 tiles): a_wg = 2048 wg, the warpgroup's 8 row groups of
+// each 4096-byte A chunk.  No fragments, so the stage itself is what must outlive the MMAs in flight.
+template <int S>
+__device__ __forceinline__ void oz_chunk_ss(uint32_t* acc, uint32_t sa, uint32_t a_wg, uint32_t acc_in) {
+  constexpr int A_BYTES = OZ_BM * OZ_KC, B_BYTES = 64 * OZ_KC;
+  const uint64_t adesc = desc_nosw(sa + a_wg), bdesc = desc_nosw(sa + S * A_BYTES);
+  wgmma_fence();
+#pragma unroll
+  for (int s = 0; s < S; ++s)
+#pragma unroll
+    for (int t = 0; t < S - s; ++t)
+      WgmmaI8SS64::mma(acc + (s + t) * 32, adesc + (uint64_t)(s * (A_BYTES >> 4)), bdesc + (uint64_t)(t * (B_BYTES >> 4)),
+                       s == 0 ? acc_in : 1u);
+  wgmma_commit();
+}
+
 // the drain of one consumer thread: rows r0, r0 + 8 of the tile and columns 8j + 2(lane & 3) + {0, 1} of every
 // accumulator block; C += sign * (2^e_i 2^e_j 2^-33) * v with rs[h] = sign 2^e_i 2^-33 (2^-28 for 8-bit digits), streamed
 // (.cs) so the int8 slices stay resident in L2.  STAGED: a full tile whose old C is in the staged block; otherwise guarded
@@ -386,22 +407,23 @@ __device__ __forceinline__ void oz_chunk(uint32_t* acc, uint32_t (&af)[S][4], ui
 template <int S, int BITS, int BN, bool PAIR32, bool STAGED, typename CT>
 __device__ __forceinline__ void oz_drain(const OzTileArgs& a, const uint32_t* acc, const CT* cbuf, int bi, int bj, int64_t brow,
                                          int r0, const double* rs) {
-  constexpr int C_LD = OzCfg<S, CT>::C_LD;
+  constexpr int C_LD = OzCfg<S, BITS, CT>::C_LD;
   CT* C = (CT*)a.C;
   const int64_t m0 = (int64_t)bi * OZ_BM + r0;
   const int cq = 2 * ((threadIdx.x & 31) & 3);
+  constexpr int RND = (BITS == 8) ? 4 : 8;  // the 192 accumulators of the eight-bit tile leave room for 4 loads in flight
 #pragma unroll
-  for (int i0 = 0; i0 < BN / 2; i0 += 8) {  // 8 elements (two 8-column groups) per round: loads first, then stores
-    double cv[8];
+  for (int i0 = 0; i0 < BN / 2; i0 += RND) {  // RND elements (one or two 8-column groups) per round: loads, then stores
+    double cv[RND];
 #pragma unroll
-    for (int i = i0; i < i0 + 8; ++i) {
+    for (int i = i0; i < i0 + RND; ++i) {
       const int c = 8 * (i >> 2) + cq + (i & 1), h = (i >> 1) & 1;
       const int64_t row = m0 + 8 * h, col = (int64_t)bj * BN + c;
       if constexpr (STAGED) cv[i - i0] = (double)cbuf[c * C_LD + r0 + 8 * h];
       else cv[i - i0] = (row < a.M && col < a.N) ? ld_cs(C + row + col * a.ldc) : 0.0;
     }
 #pragma unroll
-    for (int i = i0; i < i0 + 8; ++i) {
+    for (int i = i0; i < i0 + RND; ++i) {
       const int c = 8 * (i >> 2) + cq + (i & 1), h = (i >> 1) & 1;
       const int64_t row = m0 + 8 * h, col = (int64_t)bj * BN + c;
       const double v = oz_combine<S, BITS, BN, PAIR32>(acc, i);
@@ -417,7 +439,7 @@ __device__ __forceinline__ void oz_syrk_body(const OzTileArgs& a, int64_t ntiles
   // [b * tpc, (b + 1) * tpc) and exits; the grid is ceil(ntiles / tpc).  Bounded CTAs hand their SM back every ~0.1 ms, so
   // kernels of a higher-priority stream (the panel chain, the NCCL broadcast) are scheduled between them instead of
   // waiting for the whole update.
-  using Cfg = OzCfg<S, CT>;
+  using Cfg = OzCfg<S, BITS, CT>;
   constexpr int BN = Cfg::BN, STAGES = Cfg::STAGES, STAGE_BYTES = Cfg::STAGE_BYTES;
   constexpr int A_BYTES = Cfg::A_BYTES, B_BYTES = Cfg::B_BYTES, C_LD = Cfg::C_LD;
   const int64_t t_begin = tpc ? (int64_t)blockIdx.x * tpc : (int64_t)blockIdx.x;
@@ -501,7 +523,14 @@ __device__ __forceinline__ void oz_syrk_body(const OzTileArgs& a, int64_t ntiles
         const uint32_t st = it % STAGES, ph = (it / STAGES) & 1;
         mbar_wait(&full_bar[st], ph);
         const uint32_t sa = smem0 + st * STAGE_BYTES;
-        if constexpr (NAF == 2) {
+        if constexpr (BITS == 8) {
+          // the MMAs of chunk kb - 1 still read their stage until the wait below retires them
+          oz_chunk_ss<S>(acc, sa, 2048u * wg, kb != 0 ? 1u : 0u);
+          if (kb > 0) {
+            wgmma_wait<1>();
+            if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+          }
+        } else if constexpr (NAF == 2) {
           // the fragments of chunk kb - 2 are free: its MMAs completed at the wait below in iteration kb - 1
           if (kb & 1) oz_chunk<S, BN>(acc, af[NAF - 1], sa, a_lane, 1u);
           else oz_chunk<S, BN>(acc, af[0], sa, a_lane, kb != 0 ? 1u : 0u);
@@ -515,7 +544,7 @@ __device__ __forceinline__ void oz_syrk_body(const OzTileArgs& a, int64_t ntiles
           if (lane == 0) mbar_arrive(&empty_bar[st]);
         }
       }
-      if constexpr (NAF == 2) {
+      if constexpr (NAF == 2 || BITS == 8) {
         wgmma_wait<0>();
         if (lane == 0) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
       }
@@ -572,7 +601,7 @@ struct OzKernel<6, 8, double> {
 template <int S, int BITS, typename CT>
 int launch_syrk_wgmma(const OzakiWs& ws, void* C, int64_t ldc, int64_t M, int64_t N, int64_t b_tile_stride,
                       int64_t b_tile_width, int64_t b_off, int64_t a_off, cudaStream_t s, int full, double sign) {
-  using Cfg = OzCfg<S, CT>;
+  using Cfg = OzCfg<S, BITS, CT>;
   constexpr int BN = Cfg::BN, R = OZ_BM / BN;
   constexpr auto kernel = OzKernel<S, BITS, CT>::fn;
   static uint64_t configured = 0;  // per-device bit: the attribute is per device (one ctx per GPU in one process)
@@ -629,7 +658,8 @@ int launch_syrk_wgmma(const OzakiWs& ws, void* C, int64_t ldc, int64_t M, int64_
   if (ntiles <= 0) return 0;
   const int cap = (ws.max_ctas > 0 && ws.max_ctas < nsm) ? ws.max_ctas : nsm;
   int64_t grid = cap < ntiles ? cap : ntiles;
-  const int tpc = ws.chunk_tiles;
+  // chunk_tiles counts 128 x 32 tiles; a 128 x 64 tile (eight-bit digits) covers two, so a bounded CTA keeps its area
+  const int tpc = (BITS == 8 && ws.chunk_tiles > 1) ? ws.chunk_tiles / 2 : ws.chunk_tiles;
   if (tpc > 0) grid = (ntiles + tpc - 1) / tpc;
   kernel<<<(unsigned)grid, OZ_THREADS, Cfg::SMEM, s>>>(a, ntiles, nbi, nbj, tpc);
   agp_count_launch();
