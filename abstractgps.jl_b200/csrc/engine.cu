@@ -48,7 +48,8 @@ struct agp_ctx {
   ncclComm_t nccl = nullptr;
   OzakiWs oz{};            // slice workspace of the int8-slice fp64 path (cached across fits of the same shape)
   OzakiWs oz2{};           // second slice buffer of the pipelined distributed schedule (panel k+1 is sliced while rest(k) runs)
-  int64_t oz_rows = 0, oz2_rows = 0;
+  OzakiWs ozp{};           // slices of the first half of a two-level outer panel (K = half the panel width; cholesky_inplace)
+  int64_t oz_rows = 0, oz2_rows = 0, ozp_rows = 0;
   cudaStream_t stream_comm = nullptr;  // panel broadcasts of the pipelined distributed schedule
   int oz_S = 6;             // ozaki_slices: 6 = six 8-bit digits in the factorisation (slice_format), 5, 7, 8 = 7-bit slices
   int oz_chunk = 16;        // bounded-CTA size (tiles) of the rest updates that run beside a higher-priority stream; 0 = persistent
@@ -371,7 +372,8 @@ static void join_inverses(agp_ctx* ctx) {
 }
 
 // resolve the outer panel width (in 128-blocks) and the fp64 trailing-update engine for a problem size:
-// explicit config / env wins; "auto" = int8-sliced tensor-core path with 512-wide panels from n_pad >= 8192
+// explicit config / env wins; "auto" = int8-sliced tensor-core path with 512-wide panels from n_pad >= 8192 (the
+// single-GPU fp64 factorisation on eight-bit slices widens them to 1024 from AUTO_NB1024_MIN, see cholesky_inplace)
 static int resolve_G(const agp_ctx* ctx, int64_t n_pad) {
   int nb = ctx->cfg.tile_nb;
   if (nb <= 0) nb = (n_pad >= 8192) ? 512 : TILE;
@@ -379,6 +381,7 @@ static int resolve_G(const agp_ctx* ctx, int64_t n_pad) {
   if (G > 8) G = 8;  // kernels that stage a whole outer block (distributed backward solve) hold at most 8 inner blocks
   return G < 1 ? 1 : G;
 }
+constexpr int64_t AUTO_NB1024_MIN = 32768;  // C4h (N = 32 768) and C4 (65 536) measured faster at 1024; smaller N not measured
 static int resolve_fp64_mode(const agp_ctx* ctx, int64_t n_pad) {
   if (ctx->cfg.fp64_mode >= 0) return ctx->cfg.fp64_mode;
   return n_pad >= 8192 ? 1 : 0;
@@ -490,6 +493,28 @@ void factor_panel(agp_ctx* ctx, T* Lp, int64_t lda, int Gp, int64_t rows, T* Din
   for (int g = 0; g < Gp; ++g) factor_panel_step<T>(ctx, Lp, lda, Gp, g, rows, Dinv_p, logdet_part, blk_base, info, s);
 }
 
+// factor the outer panel of inner blocks [ko, ko + Gp) of the Cholesky at L.  With `ozp` (slices of K = Gp/2 inner
+// blocks) the panel is two-level: factor its first half, apply that half's rank-K update to the second half's columns
+// (every row below the first half: a rectangle plus the lower tiles of its diagonal block) on the int8-slice kernel,
+// then factor the second half.  The rank-128 DMMA updates inside each half then span at most Gp/2 - 1 inner blocks, as
+// in a panel of half the width, instead of Gp - 1.
+template <typename T>
+void factor_outer_panel(agp_ctx* ctx, T* L, int64_t lda, int ko, int Gp, int64_t rows_total, T* Dinv,
+                        double* logdet_part, int* info, cudaStream_t s, const OzakiWs* ozp) {
+  const int64_t p0 = (int64_t)ko * TILE;
+  if (!ozp || (int64_t)Gp * TILE != 2 * (int64_t)ozp->K) {
+    factor_panel<T>(ctx, L + p0 + p0 * lda, lda, Gp, rows_total - p0, Dinv + p0 * TILE, logdet_part, ko, info, s);
+    return;
+  }
+  const int h = Gp / 2;
+  const int64_t h0 = p0 + (int64_t)h * TILE;  // first row / column of the second half
+  factor_panel<T>(ctx, L + p0 + p0 * lda, lda, h, rows_total - p0, Dinv + p0 * TILE, logdet_part, ko, info, s);
+  constexpr int is_f32 = std::is_same<T, double>::value ? 0 : 1;
+  ozaki_prepare_ex(*ozp, L + h0 + p0 * lda, is_f32, 0, lda, rows_total - h0, 0, s);
+  trailing_update<T>(ctx, L, lda, h0, h0, p0, ozp->K, rows_total - h0, (int64_t)(Gp - h) * TILE, s, ozp, h0);
+  factor_panel<T>(ctx, L + h0 + h0 * lda, lda, Gp - h, rows_total - h0, Dinv + h0 * TILE, logdet_part, ko + h, info, s);
+}
+
 template <typename T>
 void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t rows_total, T* Dinv,
                       double* logdet_part, int* info) {
@@ -498,16 +523,26 @@ void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t ro
   const int fp64_mode = resolve_tensor_mode<T>(ctx, n_pad);  // 1: int8-sliced tensor-core trailing update (fp64: slice_format, fp32: 4 slices)
   int G = resolve_G(ctx, n_pad);
   if (!std::is_same<T, double>::value && fp64_mode == 1 && ctx->cfg.tile_nb <= 0 && n_pad >= 4096) G = 4;  // 512-wide panels
+  // fp64 on eight-bit slices: 1024-wide (two-level) panels from AUTO_NB1024_MIN, where they measured faster (DESIGN §6)
+  if (std::is_same<T, double>::value && fp64_mode == 1 && ctx->cfg.tile_nb <= 0 && ctx->oz_S == 6 &&
+      n_pad >= AUTO_NB1024_MIN)
+    G = 8;
   const bool oz_ok = fp64_mode == 1 && nblk > 2 * G && ensure_oz<T>(ctx, rows_total, G * TILE, true, s) &&
                      (std::is_same<T, double>::value || ctx->oz.bulk == 2);
+  // two-level outer panels (factor_outer_panel) where the trailing update runs on eight-bit slices and the panel is wider
+  // than 512; the in-panel slices keep their own workspace, so neither it nor the trailing one is recreated per panel
+  const OzakiWs* ozp = nullptr;
+  if (oz_ok && ctx->oz.bits == 8 && G > 4 && G % 2 == 0 &&
+      ensure_ws(ctx->ozp, ctx->ozp_rows, rows_total, G / 2 * TILE, slice_format<T>(ctx, G / 2 * TILE, true), s) &&
+      ctx->ozp.bits == 8)
+    ozp = &ctx->ozp;
   const bool la = ctx->cfg.lookahead != 0 && nblk > 2 * G;
   const bool la2 = la && ctx->cfg.lookahead >= 2;
   bool rest_pending = false, restA_pending = false, last_rest_full = false;
   size_t ev_idx = 0, last_rest = 0, last_restA = 0;
   for (int ko = 0; ko < nblk; ko += G) {
     const int g_end = (ko + G < nblk) ? ko + G : nblk;  // inner blocks [ko, g_end)
-    factor_panel<T>(ctx, L + (int64_t)ko * TILE + (int64_t)ko * TILE * lda, lda, g_end - ko, rows_total - (int64_t)ko * TILE,
-                    Dinv + (int64_t)ko * TILE * TILE, logdet_part, ko, info, s);
+    factor_outer_panel<T>(ctx, L, lda, ko, g_end - ko, rows_total, Dinv, logdet_part, info, s, ozp);
     const int64_t t0 = (int64_t)g_end * TILE;           // first trailing row/column
     const int64_t cols_trail = n_pad - t0;
     if (cols_trail <= 0) continue;
@@ -565,7 +600,9 @@ void cholesky_inplace(agp_ctx* ctx, T* L, int64_t lda, int64_t n_pad, int64_t ro
     if (cols_trail > next_cols) {
       const int64_t r0 = t0 + next_cols;
       cudaStreamWaitEvent(s2, e_panel, 0);
-      if (oz) oz->chunk_tiles = ctx->oz_chunk;  // the panel chain on the (higher-priority) main stream gets SMs between CTAs
+      // the panel chain on the (higher-priority) main stream gets SMs between CTAs.  oz_chunk is the area of a bounded CTA
+      // at K = 512; a wider panel's tile takes K / 512 times as long, so the CTA takes that many times fewer tiles
+      if (oz) oz->chunk_tiles = K > 512 && ctx->oz_chunk > 0 ? std::max(1, (int)(ctx->oz_chunk * 512 / K)) : ctx->oz_chunk;
       trailing_update<T>(ctx, L, lda, r0, r0, kc0, K, rows_total - r0, n_pad - r0, s2, oz, t0);
       if (oz) oz->chunk_tiles = 0;
       cudaEventRecord(e_rest, s2);
@@ -3641,6 +3678,7 @@ int32_t agp_destroy(agp_ctx* ctx) {
   for (auto e : ctx->dep_ev) cudaEventDestroy(e);
   if (ctx->oz.SL) ozaki_ws_destroy(&ctx->oz, ctx->stream);
   if (ctx->oz2.SL) ozaki_ws_destroy(&ctx->oz2, ctx->stream);
+  if (ctx->ozp.SL) ozaki_ws_destroy(&ctx->ozp, ctx->stream);
   if (ctx->stream_comm) { cudaStreamSynchronize(ctx->stream_comm); cudaStreamDestroy(ctx->stream_comm); }
   if (ctx->nccl) ncclCommDestroy(ctx->nccl);
   cudaEventDestroy(ctx->ev_s3);
